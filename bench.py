@@ -3,6 +3,7 @@
 metric), through the drop-in modules -> libffc_b200.so.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--math fp32|bf16x3]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 One "step" = one forward pass of the generator over one batch of 32 synthetic 512x512 (image, mask)
@@ -18,6 +19,9 @@ Reported on one JSON line by rank 0:
                with SURVEY.md §8(d)'s algorithmic bytes
   cpu_baseline the oracle's torch-CPU port (the reference's own operator sequence) on this box's host cores
 `--impl reference` times that CPU port alone (bounded sample per step) as the reference arm.
+`--dump-outputs DIR` writes what the last timed step computed (the generator output, rank 0) as DIR/<name>.npy in
+float32, a fixed sample of it when the whole would exceed 64 MB; inputs and weights are seeded, so two builds run
+with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -42,25 +46,26 @@ def _peaks():
             d = json.load(fh)
         return dict(hbm_gbs=d["hbm_gbs"], bf16_burst=d["bf16_tflops"], bf16_sustained=d["bf16_tflops_sustained"],
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, bf16_burst=1590.0, bf16_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (700 W): HBM3 3.35 TB/s, dense BF16 989 TFLOP/s — a denominator, not a reached rate
+    return dict(hbm_gbs=3350.0, bf16_burst=989.0, bf16_sustained=989.0, source="fallback (H100 SXM data sheet)")
 
 
-def _ncu_traffic(prefix):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed `ncu --set full` capture
-    (profiles/r02_traffic.json, bs32 512x512, written by tools/ncu_traffic.py; kernels that did not change since
-    round 1 fall back to profiles/r01_traffic.json); None if neither capture holds the kernel."""
-    for name in ("r02_traffic.json", "r01_traffic.json"):
-        p = os.path.join(ROOT, "profiles", name)
-        if not os.path.isfile(p):
-            continue
-        with open(p) as fh:
-            for k, v in json.load(fh).items():
-                if k.startswith(prefix):
-                    if isinstance(v, list):                       # ncu_traffic.py: one record per captured launch
-                        vals = [e["dram_bytes"] for e in v if "dram_bytes" in e]
-                        return sum(vals) / len(vals) if vals else None
-                    return v
-    return None
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(directory, outputs):
+    """Write {name: tensor} as <directory>/<name>.npy in float32.  An output larger than the 64 MB budget is
+    replaced by a fixed sample of its elements (seed 0, sorted flat indices, <name>_sample.npy)."""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    budget = DUMP_LIMIT_BYTES // max(1, len(outputs))
+    for name, t in sorted(outputs.items()):
+        a = t.detach().float().cpu().numpy()
+        if a.nbytes > budget - 4096:                  # room for the .npy header
+            n = (budget - 4096) // 4
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=n, replace=False))
+            a, name = a.reshape(-1)[idx], name + "_sample"
+        np.save(os.path.join(directory, name + ".npy"), np.ascontiguousarray(a, dtype=np.float32))
 
 
 class ClockSampler:
@@ -127,8 +132,8 @@ CPU_IMAGES_PER_STEP = 4
 def _cpu_setup():
     """Build the CPU model once.  Thread count: FIXED at min(16, available) in both arms (stated in the JSON line).
     Round 1 calibrated it per run and the two arms disagreed (8 vs 16 threads on the same box); the box reports 128
-    logical CPUs but oversubscribed intra-op pools are far slower than a right-sized one (first B200 run: 128 threads
-    -> 0.017 img/s, 16 -> 1.9 img/s, 8 -> 1.4 img/s), so "all the host threads it can use" is 16 here."""
+    logical CPUs but oversubscribed intra-op pools are far slower than a right-sized one, so "all the host threads it
+    can use" is 16 here."""
     import torch
     from lama_b200 import modules as M
     from lama_b200.testing import BIG_LAMA_KWARGS, seeded_parameters_, synthetic_image_mask, generator_input
@@ -302,6 +307,8 @@ def main():
     ap.add_argument("--no-fp32-arm", action="store_true", help="skip the CUDA-core fp32 reading of the same step")
     ap.add_argument("--no-torch-cuda-baseline", action="store_true",
                     help="skip the torch-eager (cuFFT/cuDNN) reading of the same operator sequence on this GPU")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the generator output of the last timed step as DIR/<name>.npy (float32, <= 64 MB)")
     ap.add_argument("--io", default=os.environ.get("LAMA_B200_BENCH_IO", "both"), choices=["f32", "both"],
                     help="both: also time the uint8 predict path (lama_b200.predict, SURVEY.md row f1) end to end")
     args = ap.parse_args()
@@ -381,6 +388,8 @@ def main():
     with ClockSampler(local) as clk:
         ms = timed(graphed.graph.replay, args.steps)
     clocks = clk.summary()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, ex.outputs)          # the program's outputs: the generator result
     value = world * B * args.steps / (ms / 1e3)
 
     # ---- end to end through the public serving API with HOST buffers: every step copies its pinned (B,4,S,S)
@@ -448,14 +457,13 @@ def main():
         roof = {"kernel": "conv_simt_kernel" if math == L.MATH_FP32 else "conv_tc_kernel",
                 "op": "resblock local 3x3 contraction (convl2l+convg2l+bn_l+relu): M=B*64*64, N=128, K=9*512",
                 "bound": "tensor", "achieved": ach, "peak": peaks["bf16_burst"], "unit": "TFLOP/s",
-                "frac": ach / peaks["bf16_burst"], "traffic": _ncu_traffic("L:") if (B, S) == (32, 512) else None,
-                "ms_per_launch": ms_c,
+                "frac": ach / peaks["bf16_burst"], "ms_per_launch": ms_c,
                 "algorithmic_flops_per_launch": flops, "peak_source": peaks["source"] + ", bf16 burst",
                 "ms_per_launch_hot": ms_c_hot,
                 "frac_hot_vs_sustained_peak": flops / (ms_c_hot * 1e-3) / 1e12 / peaks["bf16_sustained"],
                 "executed_over_algorithmic": 1.0 if math == L.MATH_FP32 else 3.0,
                 "note": "fp32 CUDA-core arm (FFCB_MATH_FP32)" if math == L.MATH_FP32 else
-                        "bf16x3 tcgen05 arm: 3 bf16 products per algorithmic MAC (frac <= 1/3 by construction); "
+                        "bf16x3 wgmma arm: 3 bf16 products per algorithmic MAC (frac <= 1/3 by construction); "
                         "ms_per_launch / frac: 10 launches after 2 idle seconds vs the burst peak; ms_per_launch_hot / "
                         "frac_hot_vs_sustained_peak: 10 launches right after the power-capped steps vs the back-to-back "
                         "cuBLAS figure of MEASURED_PEAKS.json"}
@@ -475,7 +483,7 @@ def main():
             run_calls(fu_calls * 3)
             c = 192
             fu_bytes = 4.0 * B * h * h * (c + c) + 4.0 * (2 * c) * (2 * c) + 8.0 * (2 * c)
-            flush = torch.empty(512 << 20, dtype=torch.uint8, device=dev)     # 4x the 126 MB L2
+            flush = torch.empty(512 << 20, dtype=torch.uint8, device=dev)     # 10x the 50 MB L2
 
             def fu_time(cold, idx):
                 """median of `reps` single runs; cold: a 512 MB write evicts L2 before every run (outside the events)"""
@@ -506,7 +514,6 @@ def main():
                                              "frac": fu_bytes / (ms_warm * 1e-3) / 1e9 / peaks["hbm_gbs"]},
                                     "per_kernel": parts,
                                     "layout": ("planar" if any(bf.cg for bf in ex.prog.bufs) else "nhwc"),
-                                    "traffic": _ncu_traffic("FU:") if (B, S) == (32, 512) else None,
                                     "note": "SURVEY.md 8(d): algorithmic bytes = t in + u out + weights; spectrum "
                                             "intermediates not counted; graded figure = cold L2"}
 
@@ -590,7 +597,7 @@ def main():
             "data": "synthetic",
             "config": {"workload": f"big-lama FFCResNetGenerator fwd (configs[2]), bs{B}/GPU {S}x{S}, seeded random weights",
                        "global_batch": B * world, "parallelism": f"batch-sharded x{world}, no data-path collective",
-                       "math": args.math, "l2": "inputs+activations (>4 GB/step) exceed the 126 MB L2; no explicit flush",
+                       "math": args.math, "l2": "inputs+activations (>4 GB/step) exceed the 50 MB L2; no explicit flush",
                        "cuda_graph": True},
             "e2e": {"value": e2e, "unit": "images/s", "h2d_bytes_per_step": x_host.numel() * 4 * 1,
                     "d2h_bytes_per_step": y_host.numel() * 4, "ms_per_step": ms_e2e / args.steps,

@@ -1,5 +1,5 @@
 /*
- * ffc_b200.h — C ABI of libffc_b200.so: the B200 (sm_100a) kernels behind the drop-in
+ * ffc_b200.h — C ABI of libffc_b200.so: the H100 (sm_90a) kernels behind the drop-in
  * replacements for advimman/lama's FFC inference path
  * (reference: saicinpainting/training/modules/ffc.py).
  *
@@ -25,7 +25,7 @@
  *    Tensors of the FourierUnit chain may instead be "channel-group planar" (ffcb_tensor.cg / .sg below).
  *  - storage formats: FFCB_F32 (float) and FFCB_BF16X2 ("split" bfloat16: value = hi + lo with
  *    hi = bf16(v), lo = bf16(v - hi); hi plane at ptr, lo plane at ptr + lo_off elements).
- *    The split format is what the tcgen05 path multiplies (3 bf16 products, fp32 accumulate:
+ *    The split format is what the wgmma path multiplies (3 bf16 products, fp32 accumulate:
  *    hi*hi + lo*hi + hi*lo, relative error ~2^-16, see DESIGN.md "precision").
  */
 #ifndef FFC_B200_H_
@@ -43,7 +43,7 @@ extern "C" {
 enum {
   FFCB_OK = 0,
   FFCB_EINVAL = -1,  /* bad shape / alignment / unsupported combination */
-  FFCB_EARCH = -2,   /* device is not sm_100 */
+  FFCB_EARCH = -2,   /* device is not sm_90 */
   FFCB_ECUDA = -3,   /* CUDA runtime / driver error (text in ffcb_last_error) */
   FFCB_ENOMEM = -4   /* caller-provided workspace too small */
 };
@@ -54,7 +54,7 @@ enum { FFCB_BORDER_ZERO = 0, FFCB_BORDER_REFLECT = 1 };
 /* arithmetic of the contraction kernels */
 enum {
   FFCB_MATH_FP32 = 0,   /* CUDA-core FFMA, fp32 operands (reference-grade path) */
-  FFCB_MATH_BF16X3 = 1  /* tcgen05.mma kind::f16 on split-bf16 operands, fp32 accumulators in TMEM */
+  FFCB_MATH_BF16X3 = 1  /* wgmma (bf16) on split-bf16 operands, fp32 accumulators in registers */
 };
 
 typedef void* ffcb_stream_t; /* cudaStream_t */
@@ -78,14 +78,14 @@ typedef struct {
                       group of cg channels is its own dense little channels-last image.  This is the layout of the
                       FourierUnit chain (SpectralTransform.conv1 -> rfft2 -> spectral conv -> irfft2 -> conv2,
                       ffc.py:145-161): one (image, group) plane set is ONE contiguous block for the plane FFT kernels
-                      and the [K/8][pixel][8] "interleaved" (no-swizzle, K-major) operand tile of tcgen05.mma. */
-  int32_t tile;    /* 0, or 128 with cg == 8: "tile-blocked" variant for tcgen05 operands — pixels are flattened
+                      and the [K/8][pixel][8] "interleaved" (no-swizzle, K-major) operand tile of wgmma. */
+  int32_t tile;    /* 0, or 128 with cg == 8: "tile-blocked" variant for wgmma operands — pixels are flattened
                       (m = (b*H + y)*W + x over the view) and stored in blocks of 128:
                         element (m, c) at ptr + (m/128)*sg + (c/8)*1024 + (m%128)*8 + c%8
                       so the [8 groups][128 pixels][8] operand tile of one 64-channel K block of one 128-pixel M tile is
                       ONE contiguous 16 KB run (a single cp.async.bulk per plane); sg = elements per 128-pixel block
                       (all groups of the allocation), sb / sy / sx are ignored.  Written by the plane FFT kernels,
-                      read by ffcb_conv (tcgen05 arm; 1x1 taps; M tiles that coincide with the blocks). */
+                      read by ffcb_conv (tensor-core arm; 1x1 taps; M tiles that coincide with the blocks). */
   int64_t sg;      /* cg > 0: stride between channel groups (elements), or between 128-pixel blocks when tile != 0 */
 } ffcb_tensor;
 
@@ -139,7 +139,7 @@ typedef struct {
 
 int ffcb_version(void);
 const char* ffcb_last_error(void);
-/* 0 if `device` is an sm_100 part this library can run on */
+/* 0 if `device` is an sm_90 part this library can run on */
 int ffcb_check_device(int device);
 void ffcb_shutdown(void);
 

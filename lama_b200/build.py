@@ -1,7 +1,7 @@
-"""In-tree build of libffc_b200.so (sm_100a only) with nvcc.
+"""In-tree build of libffc_b200.so (sm_90a only) with nvcc.
 
 ``python -m lama_b200.build`` or ``__graft_entry__.build()``.  nvcc cross-compiles without a
-GPU; the resulting ``lama_b200/libffc_b200.so`` is git-ignored but travels to the GPU box.
+GPU; the resulting ``lama_b200/libffc_b200.so`` and ``lama_b200/build/`` are git-ignored build products.
 """
 import hashlib
 import os
@@ -17,8 +17,8 @@ STAMP = LIB_PATH + ".stamp"
 OBJ_DIR = os.path.join(HERE, "build")
 
 SOURCES = ["api.cu", "fft.cu", "fft_plane.cu", "fft_plane_cg.cu", "conv_simt.cu", "conv_tc.cu", "shell.cu", "grad.cu"]
-NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ARCH + [
     "-O3", "-std=c++17", "-lineinfo", "--expt-relaxed-constexpr",
     "-Xcompiler", "-fPIC", "-shared",
 ] + os.environ.get("LAMA_B200_NVCC_EXTRA", "").split()      # experiments only (e.g. --use_fast_math A/B)
@@ -87,7 +87,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         results = list(pool.map(lambda s: _compile_one(s, verbose), SOURCES))
     if verbose:
         sys.stderr.write("".join(out for _o, out in results))
-    cmd = [_nvcc(), "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB_PATH] + [o for o, _ in results]
+    cmd = [_nvcc(), "-shared"] + ARCH + ["-o", LIB_PATH] + [o for o, _ in results]
     proc = subprocess.run(cmd, cwd=CSRC, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if proc.returncode != 0:
         raise RuntimeError("nvcc failed linking libffc_b200.so:\n" + proc.stdout[-4000:])

@@ -86,7 +86,7 @@ int fold_reflect_border(const ffcb_tensor*, const ffcb_tensor*, int, const ffcb_
 static int check_conv(const ffcb_conv_desc* d) {
   FFCB_REQUIRE(d != nullptr, "conv: null descriptor");
   int rc;
-  const bool tc = d->math == FFCB_MATH_BF16X3;     // only the tcgen05 arm understands channel-group planar views
+  const bool tc = d->math == FFCB_MATH_BF16X3;     // only the tensor-core arm understands channel-group planar views
   if ((rc = check_tensor(&d->in[0], "conv.in[0]", tc))) return rc;
   if ((rc = check_tensor(&d->out, "conv.out", tc))) return rc;
   FFCB_REQUIRE(d->weight != nullptr, "conv: null weight");
@@ -134,8 +134,8 @@ const char* ffcb_last_error(void) { return g_err; }
 int ffcb_check_device(int device) {
   cudaDeviceProp prop;
   FFCB_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    set_error("device %d is sm_%d%d; libffc_b200 is built for sm_100a only", device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error("device %d is sm_%d%d; libffc_b200 is built for sm_90a only", device, prop.major, prop.minor);
     return FFCB_EARCH;
   }
   return FFCB_OK;

@@ -1,4 +1,4 @@
-// Shared device/host helpers for libffc_b200 (sm_100a only).
+// Shared device/host helpers for libffc_b200 (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -61,7 +61,7 @@ inline View null_view() {
 }
 
 // Validation shared by entry points: 4-channel vector access everywhere.  Channel-group planar views (cg != 0) are
-// only accepted where `allow_cg` says so (the FourierUnit chain: ffcb_conv's tcgen05 arm and the plane FFT kernels).
+// only accepted where `allow_cg` says so (the FourierUnit chain: ffcb_conv's tensor-core arm and the plane FFT kernels).
 int check_tensor(const ffcb_tensor* t, const char* name, bool allow_cg = false);
 
 __host__ __device__ __forceinline__ long long pix_off(const View& v, int b, int y, int x) {
@@ -103,6 +103,11 @@ __device__ __forceinline__ void split_pair(float a, float b, unsigned& hi, unsig
   const __nv_bfloat162 l = __floats2bfloat162_rn(a - hf.x, b - hf.y);
   hi = *reinterpret_cast<const unsigned*>(&h);
   lo = *reinterpret_cast<const unsigned*>(&l);
+}
+
+// element-wise a * b + c of a float2 with one rounding per lane (the sm_90 form of __ffma2_rn: two FFMA)
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
 
 __device__ __forceinline__ float bf16_bits_to_float(unsigned short u) {
@@ -168,7 +173,7 @@ __device__ __forceinline__ float apply_act(float v, int act) {
 }
 
 // ---- L2 residency hints (createpolicy + .L2::cache_hint accesses).  The FourierUnit chain hands two spectra from
-// kernel to kernel (rfft2 -> spectral GEMM -> irfft2); they should stay in the 126 MB L2 while the planes that are
+// kernel to kernel (rfft2 -> spectral GEMM -> irfft2); they should stay in the 50 MB L2 while the planes that are
 // only streamed through (t in, u out) should not push them out: producers store intermediates with evict_last,
 // consumers read them (and everything read once) with evict_first.  FFCB_L2_HINTS=0 makes every policy "normal".
 __device__ __forceinline__ uint64_t l2_policy(int kind) {     // 0 normal, 1 evict_first, 2 evict_last
@@ -191,11 +196,6 @@ __device__ __forceinline__ void st_hint_u4(void* p, uint4 v, uint64_t pol) {
 __device__ __forceinline__ void st_hint_f4(void* p, float4 v, uint64_t pol) {
   asm volatile("st.global.L2::cache_hint.v4.f32 [%0], {%1, %2, %3, %4}, %5;" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z),
                "f"(v.w), "l"(pol) : "memory");
-}
-// 32-byte store (sm_100: STG.256): one whole sector per lane
-__device__ __forceinline__ void st_hint_f8(void* p, const float* v, uint64_t pol) {
-  asm volatile("st.global.L2::cache_hint.v8.f32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8}, %9;" ::"l"(p), "f"(v[0]),
-               "f"(v[1]), "f"(v[2]), "f"(v[3]), "f"(v[4]), "f"(v[5]), "f"(v[6]), "f"(v[7]), "l"(pol) : "memory");
 }
 __device__ __forceinline__ float2 ld_hint_f2(const void* p, uint64_t pol) {
   float2 v;

@@ -2,7 +2,7 @@
 //
 // Reference-grade arm of ffcb_conv(): fp32 operands, FFMA, fp32 accumulate — same arithmetic as
 // the reference's fp32 convolutions (ffc.py:189-196, 129, 139, 57-59) with BatchNorm folded into
-// weights/shift and bias/residual/activation fused into the epilogue.  The tcgen05 arm
+// weights/shift and bias/residual/activation fused into the epilogue.  The tensor-core arm
 // (conv_tc.cu) implements the same ffcb_conv_desc contract and is checked against this one.
 //
 // Tiling: 128 output pixels x 64 output channels per CTA, K stepped 16 channels at a time through

@@ -1,11 +1,11 @@
-// tcgen05 arm of ffcb_conv() (FFCB_MATH_BF16X3): implicit-GEMM convolution on the 5th-gen tensor
-// cores of sm_100a.
+// Tensor-core arm of ffcb_conv() (FFCB_MATH_BF16X3): implicit-GEMM convolution with the warpgroup MMA
+// (wgmma) of sm_90a.
 //
-//   D[128 pixels x BN] (fp32, TMEM)  +=  A_hi*W_hi + A_lo*W_hi + A_hi*W_lo        per 64-channel K block
+//   D[128 pixels x BN] (fp32, registers)  +=  A_hi*W_hi + A_lo*W_hi + A_hi*W_lo        per 64-channel K block
 //
 // Operands are "split bf16" (value = hi + lo, include/ffc_b200.h): three bf16 products with fp32
-// accumulation carry ~16 mantissa bits per operand (vs 8 for plain bf16, 11 for tf32) at 1.5x the
-// tensor-pipe time of one TF32 product and the same operand bytes as fp32.
+// accumulation carry ~16 mantissa bits per operand (vs 8 for plain bf16, 11 for tf32) with the same
+// operand bytes as fp32.
 //
 // Data movement: every operand tile is one TMA box (cp.async.bulk.tensor, 128-byte swizzle) —
 //   activations: 5-D map (C, W+2p, H+2p, B, plane) over the reflect-ring-padded NHWC buffer; the tile of
@@ -15,35 +15,34 @@
 //                tile-blocked inputs (ffcb_tensor.tile, the FourierUnit chain) need no map: the "interleaved"
 //                K-major operand tile [K/8][pixel][8] is one contiguous 16 KB run, fetched with a 1-D bulk copy;
 //   weights    : 3-D map (Kpad, N, plane), K-major.
-// The three products are issued as TWO MMAs per K step ("stacked": the hi and lo planes of a weight tile are adjacent
-// in a pipeline stage and read as one K-major tile of 2*BN rows): a_hi x [w_hi | w_lo] with N = 2*BN and a_lo x w_hi with
-// N = BN into the first half of the accumulator; the epilogue adds the halves (TcParams::stack).
-// Warp roles (384 threads, persistent CTAs, one per SM): warp 0 = TMA producer, warp 1 = MMA issuer (both walk the
-// pipeline in warp-uniform control flow, one lane chosen by elect.sync issues), warp 2 = TMEM allocator, warps 4-11 =
-// epilogue (TMEM -> registers -> shift / addend / activation -> split-bf16 or fp32 NHWC tiles staged for a TMA store,
-// or planar float32 stored straight from registers; the reflected ring of a whole-plane output is written here too).
-// The TMEM accumulator ring (two 256-column stages, four for narrow tiles) lets the MMA issuer run ahead of the
-// epilogue.  Template parameters select the operand / output kinds (IL, PO) and the rows-resident mode of the 7x7
-// shell layers (RR: one halo load per M tile, resident weight tiles).
+// Warp roles (384 threads, persistent CTAs, one per SM): warp 0 = TMA producer (warp-uniform control flow, one lane
+// chosen by elect.sync issues); warpgroups 1 and 2 = consumers.  Consumer g owns pixel rows [64g, 64g+64) of the
+// 128-pixel tile: per K block it issues the three products as m64nBNk16 wgmmas straight from the shared-memory stage
+// (both operands through matrix descriptors), keeps one K block of wgmmas in flight while it releases the stage
+// before, and after the last K block runs the epilogue from its registers (shift / addend / activation -> split-bf16
+// or fp32 channels-last stores, or planar float32 stores; the reflected ring of a whole-plane output is written here
+// too).  The producer runs up to `stages` K blocks ahead, so the loads of the next tile overlap the epilogue.
+// Template parameters select the operand / output kinds (IL, PO) and the rows-resident mode of the 7x7 shell layers
+// (RR: one halo load per M tile, resident weight tiles).
 #include <cuda.h>
 #include <stdlib.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 
 namespace ffcb {
 namespace {
 
-constexpr int BM = 128;          // pixels per tile (UMMA M)
+constexpr int BM = 128;          // pixels per tile (two m64 wgmma row blocks)
 constexpr int BK = 64;           // bf16 channels per K block = one 128-byte swizzle row
-constexpr int UMMA_K = 16;
-constexpr int kThreads = 384;      // 4 control warps + 8 epilogue warps
-constexpr int kEpiWarps = 8;
+constexpr int WG_K = 16;         // K of one bf16 wgmma
+constexpr int kThreads = 384;    // producer warpgroup + 2 consumer warpgroups
+constexpr int kConsumers = 256;
 constexpr int kTileABytes = BM * BK * 2;   // 16 KB per plane
 constexpr int kMaxStages = 8;
-constexpr int kAccStages = 4;     // TMEM accumulator ring: the MMA issuer may run 3 tiles ahead of the epilogue
-constexpr int kAccStride = 128;   // TMEM columns per accumulator stage (BN <= 128)
-constexpr int kBarBytes = 1024;  // mbarriers + TMEM slot, padded so that the staging tiles stay 1024-byte aligned
-constexpr int kEpiBytes = kEpiWarps * 4096;
+constexpr int kBarBytes = 1024;  // mbarriers, padded so that the stages stay 1024-byte aligned
+constexpr int kSmemLimit = 227 * 1024;     // opt-in dynamic shared memory per block on sm_90
 
 struct TcParams {
   View out, addend;
@@ -56,36 +55,24 @@ struct TcParams {
   int TW, TH, tiles_x, tiles_y;
   int stride;
   int coord_off[2];          // +1 when in[src] is mapped with its border ring
-  int obw, obh;              // epilogue store box of one warp: obw x obh pixels (obw*obh == 32)
   int nseg;
   // Tile-blocked "interleaved" A operands (ffcb_tensor.tile == 128, cg == 8; the FourierUnit chain): the operand tile
   // [8 groups][128 pixels][8 channels] of one 64-channel K block of one M tile is ONE contiguous 16 KB run per plane,
   // fetched with a single 1-D bulk copy and multiplied through a no-swizzle K-major descriptor (core matrix = 8
-  // pixels x 16 B; SBO 128 B, LBO 2048 B).  (Measured alternatives: sixteen 2 KB bulk copies of a plain group-planar
-  // tensor: +24 us on the spectral GEMM; a (8, 128, 8) tensor-map box with its 16-byte rows: +65 us.)
+  // pixels x 16 B; SBO 128 B, LBO 2048 B).
   int a_il[2];
   const unsigned short* a_ptr[2];
   long long a_sg[2], a_lo[2];     // elements per 128-pixel block, hi -> lo plane offset
   int a_tiles_per_image[2];       // spatial mode: 128-pixel blocks per image (H * W / 128)
-  int out_planar;                 // out is channel-group planar float32: stored straight from registers
+  int out_planar;                 // out is channel-group planar float32
   int ring;                       // out has a 1-pixel reflected ring: the epilogue also writes the mirrored copies
   int hints;                      // L2 residency hints for the planar (FourierUnit chain) outputs
-  // Stacked products: the weight tile's hi and lo planes are adjacent in a pipeline stage, i.e. they ARE a K-major
-  // tile of 2*BN rows — a_hi x [w_hi | w_lo] is ONE MMA with N = 2*BN (columns [0,BN) = hi.hi, [BN,2BN) = hi.lo) and
-  // a_lo x w_hi a second one with N = BN into the first half; the epilogue adds the two halves.  Same tensor work as
-  // three N = BN MMAs, but 5 operand-tile reads from shared memory per K step instead of 6 (an SS MMA with N = 128
-  // reads 8 KB per 64 cycles = the whole 128 B/clk of the SM's shared memory).  Costs accumulator stages: 2 x 256
-  // columns instead of 4 x 128.
-  int stack, acc_stride, acc_stages;
   // Rows-resident mode (template RR; the 7x7 head's row contraction and the windowed 7x7 stem): every K segment is the
   // SAME 64-channel block of one source shifted by dy only, so the activation tile is loaded ONCE per M tile as a
-  // (TH + R) x TW halo (TW = 16, TH = 8: a dy shift is a whole number of 1024-byte swizzle atoms, the MMA descriptor
-  // just starts (dy - dy0) * TW rows further down) and the (small) weight tiles of all segments stay resident in
-  // shared memory for the whole kernel.  L2 -> shared-memory traffic per tile: 56 KB instead of nseg x 32-40 KB.
+  // (TH + R) x TW halo (a dy shift is a whole number of 1024-byte swizzle atoms, the wgmma descriptor just starts
+  // (dy - dy0) * TW rows further down) and the (small) weight tiles of all segments stay resident in shared memory
+  // for the whole kernel.
   int rr_dy0, rr_a_bytes, rr_w_bytes;
-  int desc_swap;             // bring-up: exchange LBO / SBO of the no-swizzle descriptor (FFCB_TC_DESC_SWAP)
-  int debug;                 // bring-up knobs (FFCB_TC_DEBUG): 1 no global ld/st in epilogue, 2 no epilogue work,
-                             // 4 no MMA issue, 8 no activation loads
   ffcb_kseg seg[FFCB_MAX_KSEG];
 };
 
@@ -127,19 +114,6 @@ __device__ __forceinline__ void tma_load_5d(void* dst, const CUtensorMap* map, u
       ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
       : "memory");
 }
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, const void* src, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
-               ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-__device__ __forceinline__ void tma_store_5d(const CUtensorMap* map, const void* src, int c0, int c1, int c2, int c3,
-                                             int c4) {
-  asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];"
-               ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4) : "memory");
-}
-__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // 1-D bulk copy global -> shared, completion on an mbarrier (bytes: multiple of 16, both addresses 16-byte aligned)
 __device__ __forceinline__ void bulk_load(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
@@ -151,33 +125,19 @@ __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// wgmma shared-memory matrix descriptors, as (lo, hi) 32-bit words: lo = start address >> 4 (bits [0,14)) | LBO >> 4
+// (bits [16,30)); hi = SBO >> 4 (bits [32,46)) | layout type (bits [62,64): 1 = 128-byte swizzle, 0 = none).
+// Advancing along K only touches the start-address field of the low word.
+//   128-byte swizzle, K-major: rows 128 B apart, 8-row groups 1024 B apart (SBO); LBO unused (1).
+//   no swizzle ("interleaved") K-major: the tile is [K/8][128 rows][8 bf16]; a core matrix is 8 rows x 16 B = 128
+//   contiguous bytes, 8-row groups follow each other every 128 B (SBO) and the two 16-byte K chunks of one K = 16
+//   step are one slab = 2048 B apart (LBO).
+constexpr uint32_t kLoSw = 1u << 16;
+constexpr uint32_t kHiSw = (uint32_t)(1024 >> 4) | (1u << 30);
+constexpr uint32_t kLoIl = (uint32_t)(2048 >> 4) << 16;
+constexpr uint32_t kHiIl = (uint32_t)(128 >> 4);
 
-// K-major, 128-byte swizzle shared-memory matrix descriptor (sm_100: version 1).
-// rows are 128 B apart, 8-row core-matrix groups 1024 B apart (SBO); LBO unused for swizzled K-major.
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);         // start address, bits [0,14)
-  d |= (uint64_t)0 << 16;                           // leading byte offset (ignored)
-  d |= (uint64_t)(1024 >> 4) << 32;                 // stride byte offset, bits [32,46)
-  d |= (uint64_t)1 << 46;                           // descriptor version (sm_100)
-  d |= (uint64_t)2 << 61;                           // SWIZZLE_128B
-  return d;
-}
-
-// K-major, NO swizzle ("interleaved"): the tile is [K/8][128 rows][8 bf16]; a core matrix is 8 rows x 16 B = 128
-// contiguous bytes, 8-row groups follow each other every 128 B (SBO) and the two 16-byte K chunks of one UMMA_K = 16
-// step are one slab = 2048 B apart (LBO).
-__device__ __forceinline__ uint64_t make_smem_desc_nosw(uint32_t saddr, int swap) {
-  const uint64_t lbo = swap ? 128 : 2048, sbo = swap ? 2048 : 128;
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-  d |= (lbo >> 4) << 16;
-  d |= (sbo >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  return d;
-}
+__device__ __forceinline__ uint32_t desc_addr(uint32_t saddr) { return (saddr & 0x3FFFF) >> 4; }
 
 __device__ __forceinline__ uint64_t desc64(uint32_t lo, uint32_t hi) {
   uint64_t d;
@@ -197,81 +157,84 @@ __device__ __forceinline__ bool elect_one() {
   return pred != 0;
 }
 
-// kind::f16 instruction descriptor: D=f32, A=B=bf16, both K-major, M=128, N=BN.
-__device__ __forceinline__ uint32_t make_idesc(int bn) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(bn >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of the accumulator registers across a wgmma fence / wait
+template <int BN>
+__device__ __forceinline__ void fence_acc(float* d) {
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, bf16 in, fp32 accumulators: d[4j + 2h + c] = D[row 16w + lane/4 + 8h]
+// [col 8j + 2(lane%4) + c] for warp w of the warpgroup.
+__device__ __forceinline__ void wgmma_n32(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+      "}, %16, %17, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "r"(scale_d));
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
+__device__ __forceinline__ void wgmma_n64(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+      "}, %32, %33, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d));
 }
-
-// Residual (addend) row of one pixel: 32 consecutive channels as eight 16-byte loads.
-// split bf16: raw[0..3] = hi plane (64 B), raw[4..7] = lo plane; fp32: raw[0..7] = 128 B.  `left` = channels that
-// exist from this offset on (tail of N): quads beyond it are not loaded and decode to zero.
-__device__ __forceinline__ void fetch_addend(const View& a, bool on, long long off, int left, uint4* raw) {
-#pragma unroll
-  for (int i = 0; i < 8; ++i) raw[i] = make_uint4(0u, 0u, 0u, 0u);
-  if (!on) return;
-  if (a.fmt == FFCB_F32) {
-    const float* p = reinterpret_cast<const float*>(a.ptr) + off;
-#pragma unroll
-    for (int i = 0; i < 8; ++i)
-      if (4 * i < left) raw[i] = __ldg(reinterpret_cast<const uint4*>(p + 4 * i));
-  } else {
-    const unsigned short* p = reinterpret_cast<const unsigned short*>(a.ptr) + off;
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-      if (8 * i < left) {
-        raw[i] = __ldg(reinterpret_cast<const uint4*>(p + 8 * i));
-        raw[4 + i] = __ldg(reinterpret_cast<const uint4*>(p + a.lo_off + 8 * i));
-      }
-  }
+__device__ __forceinline__ void wgmma_n96(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n96k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47"
+      "}, %48, %49, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+      : "l"(da), "l"(db), "r"(scale_d));
 }
-
-__device__ __forceinline__ void decode_addend(const View& a, const uint4* raw, float* ad) {
-  if (a.fmt == FFCB_F32) {
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      ad[4 * i] = __uint_as_float(raw[i].x); ad[4 * i + 1] = __uint_as_float(raw[i].y);
-      ad[4 * i + 2] = __uint_as_float(raw[i].z); ad[4 * i + 3] = __uint_as_float(raw[i].w);
-    }
-  } else {
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const unsigned h[4] = {raw[i].x, raw[i].y, raw[i].z, raw[i].w};
-      const unsigned l[4] = {raw[4 + i].x, raw[4 + i].y, raw[4 + i].z, raw[4 + i].w};
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        ad[8 * i + 2 * k] = __uint_as_float(h[k] << 16) + __uint_as_float(l[k] << 16);
-        ad[8 * i + 2 * k + 1] = __uint_as_float(h[k] & 0xffff0000u) + __uint_as_float(l[k] & 0xffff0000u);
-      }
-    }
-  }
+__device__ __forceinline__ void wgmma_n128(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+      "}, %64, %65, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <int BN>
+__device__ __forceinline__ void wgmma_bn(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+  static_assert(BN == 32 || BN == 64 || BN == 96 || BN == 128, "N tile");
+  if constexpr (BN == 32) wgmma_n32(d, da, db, scale_d);
+  else if constexpr (BN == 64) wgmma_n64(d, da, db, scale_d);
+  else if constexpr (BN == 96) wgmma_n96(d, da, db, scale_d);
+  else wgmma_n128(d, da, db, scale_d);
 }
 
 // ------------------------------------------------------------------------------------------ kernel
@@ -296,16 +259,16 @@ __device__ __forceinline__ TileCoord tile_coord(const TcParams& p, long long m_t
   return t;
 }
 
-// IL: some K segment reads a channel-group planar ("interleaved") operand.  The instantiation without them is the
-// round-1 kernel instruction for instruction (one descriptor kind, no per-segment walk in the MMA issuer).
-// PO: the output is channel-group planar float32 (stored from registers instead of through the staging tile).
-template <bool IL, bool PO, bool RR = false>
+// IL: some K segment reads a channel-group planar ("interleaved") operand.  The instantiation without them walks the
+// whole contraction with one descriptor kind.
+// PO: the output is channel-group planar float32.
+// BN: the N tile (TcParams::BN), a compile-time wgmma shape.
+template <bool IL, bool PO, bool RR, int BN>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_tc_kernel(const __grid_constant__ TcParams p, const __grid_constant__ CUtensorMap map_in0,
-               const __grid_constant__ CUtensorMap map_in1, const __grid_constant__ CUtensorMap map_w,
-               const __grid_constant__ CUtensorMap map_out) {
+               const __grid_constant__ CUtensorMap map_in1, const __grid_constant__ CUtensorMap map_w) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve: stages of [A_hi | A_lo | W_hi | W_lo], then barriers
+  // carve: [RR: resident weights] stages of [A_hi | A_lo | W_hi | W_lo], then barriers
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const int w_bytes = p.BN * BK * 2;
   const int stage_bytes = RR ? 2 * p.rr_a_bytes : 2 * kTileABytes + 2 * w_bytes;
@@ -314,11 +277,7 @@ conv_tc_kernel(const __grid_constant__ TcParams p, const __grid_constant__ CUten
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * stage_bytes);
   uint64_t* full = bars;
   uint64_t* empty = bars + kMaxStages;
-  uint64_t* acc_full = bars + 2 * kMaxStages;
-  uint64_t* acc_empty = acc_full + kAccStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + kAccStages);
-  uint64_t* w_bar = acc_empty + kAccStages + 1;             // RR: the resident weights have landed
-  uint8_t* stage_tile = reinterpret_cast<uint8_t*>(bars) + kBarBytes;     // 8 x 4 KB epilogue staging (1024-B aligned)
+  uint64_t* w_bar = bars + 2 * kMaxStages;                 // RR: the resident weights have landed
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
@@ -326,24 +285,13 @@ conv_tc_kernel(const __grid_constant__ TcParams p, const __grid_constant__ CUten
     prefetch_tmap(&map_in0);
     prefetch_tmap(&map_in1);
     prefetch_tmap(&map_w);
-    prefetch_tmap(&map_out);
   }
   if (warp == 1 && lane == 0) {
-    for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int a = 0; a < kAccStages; ++a) { mbar_init(&acc_full[a], 1); mbar_init(&acc_empty[a], kEpiWarps * 32); }
+    for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kConsumers); }
     if constexpr (RR) mbar_init(w_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "n"(512)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   // K blocks of the whole contraction
   int total_kblocks = 0;
@@ -397,151 +345,119 @@ conv_tc_kernel(const __grid_constant__ TcParams p, const __grid_constant__ CUten
           for (int j = 0; j < nblk; ++j, ++kb) {
             mbar_wait(&empty[stage], phase ^ 1);
             if (elect_one()) {
-            uint8_t* st = smem + (size_t)stage * stage_bytes;
-            const bool skip_a = (p.debug & 8) != 0;
-            mbar_expect_tx(&full[stage], (uint32_t)(skip_a ? 2 * w_bytes : stage_bytes));
-            const int cc = g.c0 + j * BK;
-            if (skip_a) {
-            } else if (IL && il) {
-              // one contiguous 16 KB run per plane: block of this M tile, groups cc/8 .. cc/8+7
-              const long long blk = p.flat ? (tc.m0 >> 7)
-                                           : (long long)tc.b * p.a_tiles_per_image[g.src] + ((tc.y0 * p.out.W) >> 7);
-              const unsigned short* src = p.a_ptr[g.src] + blk * p.a_sg[g.src] + (long long)(cc >> 3) * 1024;
-              bulk_load(st, src, kTileABytes, &full[stage]);
-              bulk_load(st + kTileABytes, src + p.a_lo[g.src], kTileABytes, &full[stage]);
-            } else if (p.flat) {
-              tma_load_3d(st, map, &full[stage], cc, (int)tc.m0, 0);
-              tma_load_3d(st + kTileABytes, map, &full[stage], cc, (int)tc.m0, 1);
-            } else {
-              tma_load_5d(st, map, &full[stage], cc, cx, cy, tc.b, 0);
-              tma_load_5d(st + kTileABytes, map, &full[stage], cc, cx, cy, tc.b, 1);
-            }
-            tma_load_3d(st + 2 * kTileABytes, &map_w, &full[stage], kb * BK, n_tile * p.BN, 0);
-            tma_load_3d(st + 2 * kTileABytes + w_bytes, &map_w, &full[stage], kb * BK, n_tile * p.BN, 1);
+              uint8_t* st = smem + (size_t)stage * stage_bytes;
+              mbar_expect_tx(&full[stage], (uint32_t)stage_bytes);
+              const int cc = g.c0 + j * BK;
+              if (IL && il) {
+                // one contiguous 16 KB run per plane: block of this M tile, groups cc/8 .. cc/8+7
+                const long long blk = p.flat ? (tc.m0 >> 7)
+                                             : (long long)tc.b * p.a_tiles_per_image[g.src] + ((tc.y0 * p.out.W) >> 7);
+                const unsigned short* src = p.a_ptr[g.src] + blk * p.a_sg[g.src] + (long long)(cc >> 3) * 1024;
+                bulk_load(st, src, kTileABytes, &full[stage]);
+                bulk_load(st + kTileABytes, src + p.a_lo[g.src], kTileABytes, &full[stage]);
+              } else if (p.flat) {
+                tma_load_3d(st, map, &full[stage], cc, (int)tc.m0, 0);
+                tma_load_3d(st + kTileABytes, map, &full[stage], cc, (int)tc.m0, 1);
+              } else {
+                tma_load_5d(st, map, &full[stage], cc, cx, cy, tc.b, 0);
+                tma_load_5d(st + kTileABytes, map, &full[stage], cc, cx, cy, tc.b, 1);
+              }
+              tma_load_3d(st + 2 * kTileABytes, &map_w, &full[stage], kb * BK, n_tile * p.BN, 0);
+              tma_load_3d(st + 2 * kTileABytes + w_bytes, &map_w, &full[stage], kb * BK, n_tile * p.BN, 1);
             }
             __syncwarp();
             if (++stage == p.stages) { stage = 0; phase ^= 1; }
           }
         }
-      }
-    }
-  } else if (warp == 1) {
-    // ================================================================ MMA issuer
-    // All 32 lanes walk the pipeline (uniform control flow, every lane polls the barriers); ONE lane chosen by
-    // `elect.sync` issues the MMAs and commits.  Under a plain `if (lane == 0)` the compiler treats the block as
-    // divergent and wraps every UTCHMMA in an ELECT / R2UR.BROADCAST / BRA.U.ANY loop (9 instructions and two
-    // branches per 64-cycle MMA: the issuer, not the tensor pipe, set the pace); here each MMA is one uniform add
-    // plus the UTCHMMA.  Descriptors are (lo, hi) 32-bit pairs: advancing along K only touches the 14-bit
-    // start-address field of the low word.
-    {
-      const uint32_t idesc = make_idesc(p.BN), idesc2 = make_idesc(2 * p.BN);
-      constexpr uint32_t kHiSw = (uint32_t)(1024 >> 4) | (1u << 14) | (2u << 29);          // SBO 1024, v1, SWIZZLE_128B
-      const uint32_t hi_il = (uint32_t)((p.desc_swap ? 2048 : 128) >> 4) | (1u << 14);     // SBO, v1, no swizzle
-      const uint32_t lbo_il = (uint32_t)((p.desc_swap ? 128 : 2048) >> 4) << 16;           // LBO (low word)
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      if constexpr (RR) mbar_wait(w_bar, 0);
-      for (long long t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        mbar_wait(&acc_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * p.acc_stride);
-        if constexpr (RR) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          if (elect_one()) {
-            const uint32_t st = smem_u32(smem + (size_t)stage * stage_bytes);
-            const uint32_t wr = smem_u32(w_res);
-            for (int sgi = 0; sgi < ((p.debug & 4) ? 0 : p.nseg); ++sgi) {
-              const uint32_t a_off = (uint32_t)((p.seg[sgi].dy - p.rr_dy0) * p.TW * (BK * 2));
-              const uint32_t a_hi = ((st + a_off) & 0x3FFFF) >> 4;
-              const uint32_t a_lo = ((st + a_off + (uint32_t)p.rr_a_bytes) & 0x3FFFF) >> 4;
-              const uint32_t w_hi = ((wr + (uint32_t)(sgi * 2 * w_bytes)) & 0x3FFFF) >> 4;
-              const uint32_t w_lo = ((wr + (uint32_t)(sgi * 2 * w_bytes + w_bytes)) & 0x3FFFF) >> 4;
-#pragma unroll
-              for (int k = 0; k < BK / UMMA_K; ++k) {
-                const uint32_t adv = (uint32_t)((k * UMMA_K * 2) >> 4);
-                if (p.stack) {
-                  umma_bf16(d_tmem, desc64(a_hi + adv, kHiSw), desc64(w_hi + adv, kHiSw), idesc2, (sgi | k) != 0);
-                  umma_bf16(d_tmem, desc64(a_lo + adv, kHiSw), desc64(w_hi + adv, kHiSw), idesc, 1);
-                } else {
-                  umma_bf16(d_tmem, desc64(a_hi + adv, kHiSw), desc64(w_hi + adv, kHiSw), idesc, (sgi | k) != 0);
-                  umma_bf16(d_tmem, desc64(a_lo + adv, kHiSw), desc64(w_hi + adv, kHiSw), idesc, 1);
-                  umma_bf16(d_tmem, desc64(a_hi + adv, kHiSw), desc64(w_lo + adv, kHiSw), idesc, 1);
-                }
-              }
-            }
-            umma_commit(&empty[stage]);
-            umma_commit(&acc_full[acc]);
-          }
-          __syncwarp();
-          if (++stage == p.stages) { stage = 0; phase ^= 1; }
-          if (++acc == p.acc_stages) { acc = 0; acc_phase ^= 1; }
-          continue;
-        }
-        int kb = 0;
-        for (int sgi = 0; sgi < (IL ? p.nseg : 1); ++sgi) {
-          const bool il = IL && p.a_il[p.seg[sgi].src] != 0;
-          const int nblk = IL ? (p.seg[sgi].nch + BK - 1) / BK : total_kblocks;
-          const uint32_t a_hiword = il ? hi_il : kHiSw;
-          const uint32_t a_lbo = il ? lbo_il : 0u;
-          const uint32_t a_step = il ? (uint32_t)(4096 >> 4) : (uint32_t)((UMMA_K * 2) >> 4);
-          for (int j = 0; j < nblk; ++j, ++kb) {
-            mbar_wait(&full[stage], phase);
-            tc_fence_after();
-            if (elect_one()) {
-              const uint32_t st = smem_u32(smem + (size_t)stage * stage_bytes);
-              const uint32_t a_hi = ((st & 0x3FFFF) >> 4) | a_lbo;
-              const uint32_t a_lo = (((st + kTileABytes) & 0x3FFFF) >> 4) | a_lbo;
-              const uint32_t w_hi = ((st + 2 * kTileABytes) & 0x3FFFF) >> 4;
-              const uint32_t w_lo = ((st + 2 * kTileABytes + w_bytes) & 0x3FFFF) >> 4;
-#pragma unroll
-              for (int k = 0; k < BK / UMMA_K; ++k) {
-                if (p.debug & 4) break;
-                const uint32_t wadv = (uint32_t)((k * UMMA_K * 2) >> 4);     // +32 B per UMMA_K inside the swizzle row
-                const uint32_t aadv = (uint32_t)k * a_step;                  // same, or two 2048-byte slabs (interleaved)
-                if (p.stack) {
-                  umma_bf16(d_tmem, desc64(a_hi + aadv, a_hiword), desc64(w_hi + wadv, kHiSw), idesc2, (kb | k) != 0);
-                  umma_bf16(d_tmem, desc64(a_lo + aadv, a_hiword), desc64(w_hi + wadv, kHiSw), idesc, 1);
-                } else {
-                  umma_bf16(d_tmem, desc64(a_hi + aadv, a_hiword), desc64(w_hi + wadv, kHiSw), idesc, (kb | k) != 0);
-                  umma_bf16(d_tmem, desc64(a_lo + aadv, a_hiword), desc64(w_hi + wadv, kHiSw), idesc, 1);
-                  umma_bf16(d_tmem, desc64(a_hi + aadv, a_hiword), desc64(w_lo + wadv, kHiSw), idesc, 1);
-                }
-              }
-              umma_commit(&empty[stage]);                 // smem stage reusable once these MMAs retire
-              if (kb == total_kblocks - 1) umma_commit(&acc_full[acc]);
-            }
-            __syncwarp();
-            if (++stage == p.stages) { stage = 0; phase ^= 1; }
-          }
-        }
-        if (++acc == p.acc_stages) { acc = 0; acc_phase ^= 1; }
       }
     }
   } else if (warp >= 4) {
-    // ================================================================ epilogue (8 warps)
-    // lane == accumulator row == pixel.  Per 32-column chunk: TMEM -> registers, + shift (+ residual),
-    // activation, convert to the output storage (split bf16 hi|lo or fp32) and write the lane's row into
-    // a swizzled 4 KB staging tile; one elected lane then issues ONE TMA store for the warp's
-    // 32-pixel x 32-channel box.  The output tensor map does all address arithmetic, clips partial
-    // tiles / channel tails, and keeps this code small (the kernel is instruction-fetch sensitive).
-    // Warps e and e+4 share a TMEM lane quarter and alternate over the chunks.
-    const int e = warp - 4;
-    const int wq = e & 3;                    // TMEM lane quarter (== warp id % 4, the hardware rule)
-    const int half = e >> 2;
-    uint8_t* stg = stage_tile + (size_t)e * 4096;
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    // ================================================================ consumers (2 warpgroups)
+    const int g = (warp >> 2) - 1;                 // row block: pixels [64g, 64g + 64) of the tile
+    const int w = warp & 3, q = lane & 3;
+    // after the pair exchange below, this thread owns ONE pixel row of the tile and 4 consecutive channels of every
+    // 8-column group of the accumulator: even lanes row 16w + lane/4, odd lanes the row 8 below
+    const int row = g * 64 + w * 16 + (lane >> 2) + 8 * (q & 1);
+    const int cb = 4 * (q >> 1);
+    const bool odd = (q & 1) != 0;
+    const uint32_t a_row_sw = (uint32_t)(g * 64 * BK * 2) >> 4;     // 64 rows of 128 B down the swizzled tile
+    const uint32_t a_row_il = (uint32_t)(g * 64 * 16) >> 4;         // 64 rows of 16 B down one interleaved slab
     const int HW = p.out.H * p.out.W;
-    const bool has_add = p.addend.ptr != nullptr && !(p.debug & 1);
-    const bool out_split = p.out.fmt == FFCB_BF16X2;
+    const bool has_add = p.addend.ptr != nullptr;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int stage = 0;
+    uint32_t phase = 0;
+    if constexpr (RR) mbar_wait(w_bar, 0);
     for (long long t = blockIdx.x; t < num_tiles; t += gridDim.x) {
       const int n_tile = (int)(t % p.num_n_tiles);
       const TileCoord tc = tile_coord(p, t / p.num_n_tiles);
-      // this lane's pixel (for the residual load) and this warp's store box origin
-      const int row = wq * 32 + lane;
+      fence_acc<BN>(acc);
+      if constexpr (RR) {
+        mbar_wait(&full[stage], phase);
+        const uint32_t st = smem_u32(smem + (size_t)stage * stage_bytes);
+        const uint32_t wr = smem_u32(w_res);
+        for (int sgi = 0; sgi < p.nseg; ++sgi) {
+          wgmma_fence();
+          const uint32_t a_off = (uint32_t)((p.seg[sgi].dy - p.rr_dy0) * p.TW * (BK * 2));
+          const uint32_t a_hi = desc_addr(st + a_off) + a_row_sw;
+          const uint32_t a_lo = desc_addr(st + a_off + (uint32_t)p.rr_a_bytes) + a_row_sw;
+          const uint32_t w_hi = desc_addr(wr + (uint32_t)(sgi * 2 * w_bytes));
+          const uint32_t w_lo = desc_addr(wr + (uint32_t)(sgi * 2 * w_bytes + w_bytes));
+#pragma unroll
+          for (int k = 0; k < BK / WG_K; ++k) {
+            const uint32_t adv = (uint32_t)((k * WG_K * 2) >> 4);
+            wgmma_bn<BN>(acc, desc64((a_hi + adv) | kLoSw, kHiSw), desc64((w_hi + adv) | kLoSw, kHiSw), (sgi | k) != 0);
+            wgmma_bn<BN>(acc, desc64((a_lo + adv) | kLoSw, kHiSw), desc64((w_hi + adv) | kLoSw, kHiSw), 1);
+            wgmma_bn<BN>(acc, desc64((a_hi + adv) | kLoSw, kHiSw), desc64((w_lo + adv) | kLoSw, kHiSw), 1);
+          }
+          wgmma_commit();
+          wgmma_wait<1>();
+        }
+        wgmma_wait<0>();
+        fence_acc<BN>(acc);
+        mbar_arrive(&empty[stage]);
+        if (++stage == p.stages) { stage = 0; phase ^= 1; }
+      } else {
+        // one loop over the K blocks of the whole contraction; IL: the segment (and with it the descriptor kind of
+        // the A operand) is tracked alongside
+        int prev = -1, sgi = 0, j = 0;
+        for (int kb = 0; kb < total_kblocks; ++kb) {
+          const bool il = IL && p.a_il[p.seg[sgi].src] != 0;
+          const uint32_t a_lodesc = il ? kLoIl : kLoSw, a_hidesc = il ? kHiIl : kHiSw;
+          const uint32_t a_row = il ? a_row_il : a_row_sw;
+          const uint32_t a_step = il ? (uint32_t)(4096 >> 4) : (uint32_t)((WG_K * 2) >> 4);   // 2 slabs / +32 B
+          if (IL && ++j == (p.seg[sgi].nch + BK - 1) / BK) { ++sgi; j = 0; }
+          mbar_wait(&full[stage], phase);
+          wgmma_fence();
+          const uint32_t st = smem_u32(smem + (size_t)stage * stage_bytes);
+          const uint32_t a_hi = desc_addr(st) + a_row;
+          const uint32_t a_lo = desc_addr(st + kTileABytes) + a_row;
+          const uint32_t w_hi = desc_addr(st + 2 * kTileABytes);
+          const uint32_t w_lo = desc_addr(st + 2 * kTileABytes + w_bytes);
+#pragma unroll
+          for (int k = 0; k < BK / WG_K; ++k) {
+            const uint32_t wadv = (uint32_t)((k * WG_K * 2) >> 4);     // +32 B per K = 16 inside the swizzle row
+            const uint32_t aadv = (uint32_t)k * a_step;
+            wgmma_bn<BN>(acc, desc64((a_hi + aadv) | a_lodesc, a_hidesc), desc64((w_hi + wadv) | kLoSw, kHiSw),
+                         (kb | k) != 0);
+            wgmma_bn<BN>(acc, desc64((a_lo + aadv) | a_lodesc, a_hidesc), desc64((w_hi + wadv) | kLoSw, kHiSw), 1);
+            wgmma_bn<BN>(acc, desc64((a_hi + aadv) | a_lodesc, a_hidesc), desc64((w_lo + wadv) | kLoSw, kHiSw), 1);
+          }
+          wgmma_commit();
+          // the wgmmas of the previous K block have retired: its stage goes back to the producer
+          wgmma_wait<1>();
+          if (prev >= 0) mbar_arrive(&empty[prev]);
+          prev = stage;
+          if (++stage == p.stages) { stage = 0; phase ^= 1; }
+        }
+        wgmma_wait<0>();
+        fence_acc<BN>(acc);
+        mbar_arrive(&empty[prev]);
+      }
+
+      // ---- epilogue: this thread's pixel
       int b, y, x;
       bool valid;
       if (p.flat) {
@@ -558,151 +474,51 @@ conv_tc_kernel(const __grid_constant__ TcParams p, const __grid_constant__ CUten
         x = tc.x0 + row % p.TW;
         valid = y < p.out.H && x < p.out.W;
       }
+      const long long o_out = valid ? pix_off(p.out, b, y, x) : 0;
       const long long o_add = (has_add && valid) ? pix_off(p.addend, b, y, x) : 0;
-      // this pixel's mirror images in the output's reflected ring, as element offsets from the pixel itself (0: none)
+      // this pixel's mirror images in the output's reflected ring, as element offsets from the pixel itself (0: none):
+      // pixels of rows 1 / H-2 and columns 1 / W-2 also land on the ring (<= 3 copies) — no separate ring kernel
       int mir_dy = 0, mir_dx = 0;
-      if (!PO && p.ring && valid && !(p.debug & 1)) {
+      if (!PO && p.ring && valid) {
         int my, mx;
         if (ring_mirrors(p.out, y, x, my, mx)) {
           if (my != -2) mir_dy = (my - y) * (int)p.out.sy;
           if (mx != -2) mir_dx = (mx - x) * (int)p.out.sx;
         }
       }
-      const int box_x = tc.x0 + (wq * 32) % p.TW, box_y = tc.y0 + (wq * 32) / p.TW;
-      const int c_end = (p.debug & 2) ? 0 : p.BN;
-
-      // residual rows do not depend on the accumulator: request the first chunk's before waiting for the MMAs,
-      // and each following chunk's while the current one is converted and stored (eight 16-byte loads per lane)
-      uint4 raw[8];
-      fetch_addend(p.addend, has_add && valid && half * 32 < c_end, o_add + n_tile * p.BN + half * 32,
-                   p.N - (n_tile * p.BN + half * 32), raw);
-      mbar_wait(&acc_full[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + ((uint32_t)(wq * 32) << 16) + (uint32_t)(acc * p.acc_stride);
-      for (int c0 = half * 32; c0 < c_end; c0 += 64) {
-        const int n0 = n_tile * p.BN + c0;
-        // residual / addend row of this pixel (32 channels) was requested one chunk ahead: raw[] holds it
-        float ad[32];
-        decode_addend(p.addend, raw, ad);
-        uint32_t r[32];
-        tmem_ld32(t_row + (uint32_t)c0, r);
-        if (p.stack) {       // + the a_hi x w_lo half of the stacked accumulator
-          uint32_t r2[32];
-          tmem_ld32(t_row + (uint32_t)(p.BN + c0), r2);
+      const uint64_t pol = l2_policy(PO && p.hints ? 2 : 0);      // planar outputs: consumed by the next kernel
 #pragma unroll
-          for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(__uint_as_float(r[j]) + __uint_as_float(r2[j]));
+      for (int j = 0; j < BN / 8; ++j) {
+        // lane pairs swap half of their 8-column group: even lanes keep row r, odd lanes row r + 8
+        const float s0 = odd ? acc[4 * j] : acc[4 * j + 2], s1 = odd ? acc[4 * j + 1] : acc[4 * j + 3];
+        const float r0 = __shfl_xor_sync(0xffffffffu, s0, 1), r1 = __shfl_xor_sync(0xffffffffu, s1, 1);
+        float4 v = odd ? make_float4(r0, r1, acc[4 * j + 2], acc[4 * j + 3])
+                       : make_float4(acc[4 * j], acc[4 * j + 1], r0, r1);
+        const int n = n_tile * p.BN + 8 * j + cb;
+        if (!valid || n >= p.N) continue;
+        if (p.shift != nullptr) {
+          const float4 sh = __ldg(reinterpret_cast<const float4*>(p.shift + n));
+          v.x += sh.x; v.y += sh.y; v.z += sh.z; v.w += sh.w;
         }
-        fetch_addend(p.addend, has_add && valid && c0 + 64 < c_end, o_add + n0 + 64, p.N - (n0 + 64), raw);
-        float v[32];
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          float4 sh = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (p.shift != nullptr && n0 + 4 * q < p.N) sh = __ldg(reinterpret_cast<const float4*>(p.shift + n0 + 4 * q));
-          v[4 * q] = __uint_as_float(r[4 * q]) + sh.x;
-          v[4 * q + 1] = __uint_as_float(r[4 * q + 1]) + sh.y;
-          v[4 * q + 2] = __uint_as_float(r[4 * q + 2]) + sh.z;
-          v[4 * q + 3] = __uint_as_float(r[4 * q + 3]) + sh.w;
-        }
-        if (!p.addend_post) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] += ad[j];
-        }
+        float4 ad = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (has_add) ad = load4(p.addend, o_add + n);
+        if (!p.addend_post) { v.x += ad.x; v.y += ad.y; v.z += ad.z; v.w += ad.w; }
         if (p.act == FFCB_ACT_RELU) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
+          v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
         } else if (p.act != FFCB_ACT_NONE) {
-          for (int j = 0; j < 32; ++j) v[j] = slow_act(v[j], p.act);
+          v.x = slow_act(v.x, p.act); v.y = slow_act(v.y, p.act); v.z = slow_act(v.z, p.act); v.w = slow_act(v.w, p.act);
         }
-        if (p.addend_post) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] += ad[j];
-        }
+        if (p.addend_post) { v.x += ad.x; v.y += ad.y; v.z += ad.z; v.w += ad.w; }
         if constexpr (PO) {
-          // channel-group planar float32 output (FourierUnit chain): the lane's pixel is contiguous with its
-          // neighbours' inside every channel group, so plain 16-byte stores are whole lines — no staging tile.
-          // (A tensor-map store with 16 / 32-byte boxes was measured 2.5x slower than these stores.)
-          if (valid && !(p.debug & 1)) {
-            float* ob = reinterpret_cast<float*>(p.out.ptr) + pix_off(p.out, b, y, x);
-            const uint64_t pol = l2_policy(p.hints ? 2 : 0);       // consumed by the next kernel of the chain
-            if (p.out.cg == 8) {                                     // 32 B per lane and group: whole sectors
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                const int n = n0 + 8 * q;
-                if (n < p.N) st_hint_f8(ob + (long long)(n >> 3) * p.out.sg, v + 8 * q, pol);
-              }
-            } else {
-#pragma unroll
-              for (int q = 0; q < 8; ++q) {
-                const int n = n0 + 4 * q;
-                if (n < p.N)
-                  st_hint_f4(ob + (long long)(n >> 2) * p.out.sg,
-                             make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]), pol);
-              }
-            }
-          }
-          continue;
-        }
-        // the previous TMA store of this warp must have finished reading the staging tile
-        if (elect_one()) tma_store_wait_read();     // (elect.sync is deterministic: always the lane that committed)
-        __syncwarp();
-        if (out_split) {
-          // [plane][32 rows][32 bf16] = 64-byte rows, TMA SWIZZLE_64B: 16-byte chunk c of row r lives at c ^ ((r>>1)&3)
-          uint4* hi = reinterpret_cast<uint4*>(stg) + lane * 4;
-          uint4* lo = reinterpret_cast<uint4*>(stg + 2048) + lane * 4;
-          const int sw = (lane >> 1) & 3;
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            unsigned h[4], l[4];
-#pragma unroll
-            for (int k = 0; k < 4; ++k) split_pair(v[8 * c + 2 * k], v[8 * c + 2 * k + 1], h[k], l[k]);
-            const uint4 h4 = make_uint4(h[0], h[1], h[2], h[3]), l4 = make_uint4(l[0], l[1], l[2], l[3]);
-            hi[c ^ sw] = h4;
-            lo[c ^ sw] = l4;
-            if ((mir_dy | mir_dx) != 0 && n0 + 8 * c < p.N) {
-              // reflected ring of the output (it feeds a 3x3 reflect contraction next): pixels of rows 1 / H-2 and
-              // columns 1 / W-2 also land on the ring (<= 3 copies, 16-byte stores) — no separate ring kernel
-              unsigned short* ob = reinterpret_cast<unsigned short*>(p.out.ptr) + pix_off(p.out, b, y, x) + (n0 + 8 * c);
-              if (mir_dy) {
-                *reinterpret_cast<uint4*>(ob + mir_dy) = h4;
-                *reinterpret_cast<uint4*>(ob + mir_dy + p.out.lo_off) = l4;
-              }
-              if (mir_dx) {
-                *reinterpret_cast<uint4*>(ob + mir_dx) = h4;
-                *reinterpret_cast<uint4*>(ob + mir_dx + p.out.lo_off) = l4;
-              }
-              if (mir_dy && mir_dx) {
-                *reinterpret_cast<uint4*>(ob + mir_dy + mir_dx) = h4;
-                *reinterpret_cast<uint4*>(ob + mir_dy + mir_dx + p.out.lo_off) = l4;
-              }
-            }
-          }
+          st_hint_f4(reinterpret_cast<float*>(p.out.ptr) + o_out + chan_off(p.out, n), v, pol);
         } else {
-          // [32 rows][32 floats] = 128-byte rows, TMA SWIZZLE_128B: chunk c of row r lives at c ^ (r & 7)
-          float4* dst = reinterpret_cast<float4*>(stg) + lane * 8;
-          const int sw = lane & 7;
-#pragma unroll
-          for (int c = 0; c < 8; ++c) dst[c ^ sw] = make_float4(v[4 * c], v[4 * c + 1], v[4 * c + 2], v[4 * c + 3]);
-        }
-        fence_async_smem();
-        __syncwarp();
-        if (!(p.debug & 1) && elect_one()) {
-          if (p.flat) tma_store_3d(&map_out, stg, n0, (int)tc.m0 + wq * 32, 0);
-          else tma_store_5d(&map_out, stg, n0, box_x, box_y, tc.b, 0);
-          tma_store_commit();
+          store4(p.out, o_out + n, v);
+          if (mir_dy) store4(p.out, o_out + mir_dy + n, v);
+          if (mir_dx) store4(p.out, o_out + mir_dx + n, v);
+          if (mir_dy && mir_dx) store4(p.out, o_out + mir_dy + mir_dx + n, v);
         }
       }
-      tc_fence_before();
-      mbar_arrive(&acc_empty[acc]);
-      if (++acc == p.acc_stages) { acc = 0; acc_phase ^= 1; }
     }
-    if (elect_one()) tma_store_wait_all();
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512) : "memory");
   }
 }
 
@@ -742,15 +558,14 @@ int encode_typed(CUtensorMap* map, void* base, CUtensorMapDataType dt, CUtensorM
   return FFCB_OK;
 }
 
-// N-tile width.  Pipeline depth matters more than tile area here: every stage carries 32 KB of
-// activations (hi+lo) plus 256 B per output column, so BN=128 leaves 3 stages in flight, BN>=192 only 2
-// (measured: 74% vs 35% tensor-pipe utilisation, profiles/r01_launches_bf16x3_v1.txt).
 int encode(CUtensorMap* map, void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
            const cuuint32_t* box, const cuuint32_t* estr, const char* what) {
   return encode_typed(map, base, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, CU_TENSOR_MAP_SWIZZLE_128B, rank, dims, strides_bytes,
                       box, estr, what);
 }
 
+// N-tile width (one wgmma N, at most 128).  Pipeline depth matters more than tile area here: every stage carries 32 KB
+// of activations (hi+lo) plus 256 B per output column, so BN=128 leaves 3 stages in flight in 227 KB, BN>=192 only 2.
 int pick_bn(int n) {
   if (const char* e = getenv("FFCB_TC_BN")) {          // tuning knob: force the N tile (multiple of 32, <= 128)
     const int v = atoi(e);
@@ -807,15 +622,10 @@ int conv_tc(const ffcb_conv_desc* d, cudaStream_t stream) {
   if (d->out.cg != 0)
     FFCB_REQUIRE(d->out.fmt == FFCB_F32 && d->out.sx % 4 == 0 && d->out.sy % 4 == 0 && d->out.sb % 4 == 0,
                  "conv(tc): channel-group planar outputs are float32");
-  if (d->out.cg == 8)     // 32-byte stores
-    FFCB_REQUIRE(d->out.sx % 8 == 0 && d->out.sy % 8 == 0 && d->out.sb % 8 == 0 && d->out.sg % 8 == 0 &&
-                     (reinterpret_cast<uintptr_t>(d->out.ptr) & 31) == 0,
-                 "conv(tc): cg = 8 planar output needs 32-byte aligned pixels");
-  {
-    const char* sw = getenv("FFCB_TC_DESC_SWAP");
-    p.desc_swap = sw ? atoi(sw) : 0;
-    p.hints = l2_hints_enabled() ? 1 : 0;
-  }
+  if (d->out.cg != 0)     // 16-byte stores
+    FFCB_REQUIRE(d->out.sg % 4 == 0 && (reinterpret_cast<uintptr_t>(d->out.ptr) & 15) == 0,
+                 "conv(tc): planar output needs 16-byte aligned channel groups");
+  p.hints = l2_hints_enabled() ? 1 : 0;
   p.addend = d->addend.ptr ? make_view(d->addend) : null_view();
   p.shift = d->shift;
   p.N = d->n_out; p.act = d->act; p.addend_post = d->addend_post;
@@ -823,23 +633,10 @@ int conv_tc(const ffcb_conv_desc* d, cudaStream_t stream) {
   p.num_n_tiles = (d->n_out + p.BN - 1) / p.BN;
   p.stride = d->stride;
   p.nseg = d->nseg;
-  {
-    const char* dbg = getenv("FFCB_TC_DEBUG");
-    p.debug = dbg ? atoi(dbg) : 0;
-  }
   int kpad = 0;
   for (int i = 0; i < d->nseg; ++i) {
     p.seg[i] = d->seg[i];
     kpad += (d->seg[i].nch + BK - 1) / BK * BK;
-  }
-  {
-    // stacked products (default; measured +3.4 % on the whole generator step, every contraction of a block gains,
-    // the short-K ones included); FFCB_TC_STACK=0 keeps three N = BN MMAs and four 128-column accumulator stages
-    const char* e = getenv("FFCB_TC_STACK");
-    p.stack = e ? (atoi(e) != 0) : 1;
-    // accumulator ring: a stacked accumulator is 2*BN columns wide — narrow tiles keep four stages
-    p.acc_stride = !p.stack ? kAccStride : (2 * p.BN <= 64 ? 64 : (2 * p.BN <= 128 ? 128 : 256));
-    p.acc_stages = 512 / p.acc_stride < kAccStages ? 512 / p.acc_stride : kAccStages;
   }
 
   // ---- tiling: flat when every tap is (0,0) on dense unit-stride inputs, else spatial TW x TH
@@ -860,8 +657,6 @@ int conv_tc(const ffcb_conv_desc* d, cudaStream_t stream) {
     p.a_tiles_per_image[s] = (t.H * t.W) >> 7;
     FFCB_REQUIRE(t.lo_off % 8 == 0, "conv(tc): tile-blocked in[%d]: lo plane not 16-byte aligned", s);
   }
-  // the epilogue stores 32-pixel boxes through a tensor map: a flattened pixel axis needs a dense output too
-  flat = flat && (d->out.cg != 0 || (d->out.sy == (int64_t)W * d->out.sx && d->out.sb == (int64_t)H * d->out.sy));
   p.flat = flat ? 1 : 0;
   // rows-resident mode (TcParams::rr_*): every segment = the same 64-channel block of one channels-last source, shifted
   // by dy only (the 7x7 head's row contraction, the windowed 7x7 stem); FFCB_TC_ROWS=0 disables it
@@ -912,11 +707,9 @@ int conv_tc(const ffcb_conv_desc* d, cudaStream_t stream) {
       FFCB_REQUIRE(p.TW == W && p.TW * p.TH == BM && H % p.TH == 0 && (H * W) % BM == 0,
                    "conv(tc): tile-blocked in[%d] in a spatial contraction needs M tiles of whole rows (W a power of two "
                    "<= 128 dividing 128, H*W a multiple of 128); got %dx%d", s, H, W);
-  p.obw = p.TW < 32 ? p.TW : 32;
-  p.obh = 32 / p.obw;
 
   // ---- tensor maps
-  alignas(64) CUtensorMap maps[4];
+  alignas(64) CUtensorMap maps[3];
   int rc;
   for (int s = 0; s < 2; ++s) {
     if (!used[s]) { p.coord_off[s] = 0; continue; }     // no tensor map: patched with a valid one below
@@ -954,55 +747,45 @@ int conv_tc(const ffcb_conv_desc* d, cudaStream_t stream) {
 
   for (int s = 0; s < 2; ++s)
     if (!used[s] || p.a_il[s]) maps[s] = maps[2];      // never dereferenced by the kernel, but prefetched
-  if (d->out.cg != 0) {
-    maps[3] = maps[2];                                   // planar outputs are stored with plain vector stores
-  } else {
-    // output: fp32 rows of 128 B (SWIZZLE_128B) or split bf16 rows of 64 B per plane (SWIZZLE_64B)
+  if (d->out.cg == 0) {
     const ffcb_tensor& t = d->out;
-    const bool split = t.fmt == FFCB_BF16X2;
-    const cuuint64_t esz = split ? 2 : 4;
+    const cuuint64_t esz = t.fmt == FFCB_BF16X2 ? 2 : 4;
     FFCB_REQUIRE(((uintptr_t)t.ptr % 16) == 0 && (t.sx * esz) % 16 == 0 && (t.sy * esz) % 16 == 0 &&
-                     (t.sb * esz) % 16 == 0 && (!split || (t.lo_off * esz) % 16 == 0),
-                 "conv(tc): out strides / pointer not 16-byte aligned (C must be a multiple of %d)", split ? 8 : 4);
-    const CUtensorMapDataType dt = split ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
-    const CUtensorMapSwizzle sw = split ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
-    if (flat) {
-      cuuint64_t dims[3] = {(cuuint64_t)t.C, (cuuint64_t)t.B * t.H * t.W, (cuuint64_t)(split ? 2 : 1)};
-      cuuint64_t str[2] = {(cuuint64_t)t.sx * esz, (cuuint64_t)(split ? t.lo_off * esz : (cuuint64_t)t.sx * esz * t.B * t.H * t.W)};
-      cuuint32_t box[3] = {32, 32, (cuuint32_t)(split ? 2 : 1)}, es[3] = {1, 1, 1};
-      if ((rc = encode_typed(&maps[3], t.ptr, dt, sw, 3, dims, str, box, es, "flat output"))) return rc;
-    } else {
-      cuuint64_t dims[5] = {(cuuint64_t)t.C, (cuuint64_t)t.W, (cuuint64_t)t.H, (cuuint64_t)t.B, (cuuint64_t)(split ? 2 : 1)};
-      cuuint64_t str[4] = {(cuuint64_t)t.sx * esz, (cuuint64_t)t.sy * esz, (cuuint64_t)t.sb * esz,
-                           (cuuint64_t)(split ? t.lo_off * esz : (cuuint64_t)t.sb * esz * t.B)};
-      cuuint32_t box[5] = {32, (cuuint32_t)p.obw, (cuuint32_t)p.obh, 1, (cuuint32_t)(split ? 2 : 1)};
-      cuuint32_t es[5] = {1, 1, 1, 1, 1};
-      if ((rc = encode_typed(&maps[3], t.ptr, dt, sw, 5, dims, str, box, es, "spatial output"))) return rc;
-    }
+                     (t.sb * esz) % 16 == 0 && (esz == 4 || (t.lo_off * esz) % 16 == 0),
+                 "conv(tc): out strides / pointer not 16-byte aligned (C must be a multiple of %d)", esz == 2 ? 8 : 4);
   }
 
   // ---- launch
   const int stage_bytes = rr ? 2 * p.rr_a_bytes : 2 * kTileABytes + 2 * p.BN * BK * 2;
-  const int bar_bytes = kBarBytes + kEpiBytes + (rr ? p.rr_w_bytes : 0);
-  int stages = (227 * 1024 - 1024 - bar_bytes) / stage_bytes;
+  const int bar_bytes = kBarBytes + (rr ? p.rr_w_bytes : 0);
+  int stages = (kSmemLimit - 1024 - bar_bytes) / stage_bytes;
   if (stages > kMaxStages) stages = kMaxStages;
   FFCB_REQUIRE(stages >= 2, "conv(tc): BN=%d leaves fewer than 2 pipeline stages", p.BN);
   p.stages = stages;
   const size_t smem = (size_t)stages * stage_bytes + bar_bytes + 1024;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   FFCB_CUDA(cudaGetDevice(&dev));
   FFCB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const long long tiles = p.num_m_tiles * p.num_n_tiles;
   const int grid = (int)(tiles < sms ? tiles : sms);
-  const bool any_il = p.a_il[0] || p.a_il[1] || getenv("FFCB_TC_FORCE_IL") != nullptr;   // (knob: A/B of the two instantiations)
+  const bool any_il = p.a_il[0] || p.a_il[1];
   auto launch = [&](auto kernel) -> int {
-    FFCB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    kernel<<<grid, kThreads, smem, stream>>>(p, maps[0], maps[1], maps[2], maps[3]);
+    FFCB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
+    kernel<<<grid, kThreads, smem, stream>>>(p, maps[0], maps[1], maps[2]);
     return FFCB_OK;
   };
-  if (rr) rc = launch(conv_tc_kernel<false, false, true>);
-  else if (any_il) rc = p.out_planar ? launch(conv_tc_kernel<true, true>) : launch(conv_tc_kernel<true, false>);
-  else rc = p.out_planar ? launch(conv_tc_kernel<false, true>) : launch(conv_tc_kernel<false, false>);
+  auto launch_bn = [&](auto bn) -> int {
+    constexpr int N = decltype(bn)::value;
+    if (rr) return launch(conv_tc_kernel<false, false, true, N>);
+    if (any_il) return p.out_planar ? launch(conv_tc_kernel<true, true, false, N>) : launch(conv_tc_kernel<true, false, false, N>);
+    return p.out_planar ? launch(conv_tc_kernel<false, true, false, N>) : launch(conv_tc_kernel<false, false, false, N>);
+  };
+  switch (p.BN) {
+    case 32: rc = launch_bn(std::integral_constant<int, 32>()); break;
+    case 64: rc = launch_bn(std::integral_constant<int, 64>()); break;
+    case 96: rc = launch_bn(std::integral_constant<int, 96>()); break;
+    default: rc = launch_bn(std::integral_constant<int, 128>()); break;
+  }
   if (rc) return rc;
   FFCB_LAUNCH_CHECK("conv_tc_kernel");
   return FFCB_OK;

@@ -4,6 +4,7 @@
 //
 // Data layout: data[point * LS + lane], LS = lane stride (32 on the device: lane == channel).
 #pragma once
+#include <math.h>
 #include <vector_functions.h>
 #include <vector_types.h>
 
@@ -16,25 +17,14 @@
 namespace ffcb {
 namespace fftc {
 
-// Complex arithmetic.  On sm_100 the (re, im) pair is one 64-bit register pair and add / sub / multiply are the packed
-// FADD2 / FMUL2 / FFMA2 instructions (two fp32 results per issue slot; negation, the re<->im swap of a multiplication
-// by +-i and scalar broadcast are operand modifiers — `FADD2 R6, R6.F32x2.HI_LO, R6.F32x2.LO_HI.NP`), which halves the
-// floating-point instruction count of the butterflies.  Every operation is still an IEEE round-to-nearest fp32 add /
-// mul / fma, so the host build (tests/host_emul) computes the same values up to fma contraction.
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ >= 1000) && !defined(FFCB_NO_F32X2)
-#define FFCB_F32X2 1
-FFCB_HD float2 cadd(float2 a, float2 b) { return __fadd2_rn(a, b); }
-FFCB_HD float2 csub(float2 a, float2 b) { return __fadd2_rn(a, make_float2(-b.x, -b.y)); }
+// Complex arithmetic: IEEE round-to-nearest fp32 add / mul / fma.  The multiply rounds a.x*b first and fuses the
+// a.y term into it, so every build (and the host emulation in tests/host_emul) rounds the same way.
 FFCB_HD float2 cmul(float2 a, float2 b) {
-  return __ffma2_rn(make_float2(-a.y, a.y), make_float2(b.y, b.x), __fmul2_rn(make_float2(a.x, a.x), b));
+  return make_float2(fmaf(-a.y, b.y, a.x * b.x), fmaf(a.y, b.x, a.x * b.y));
 }
-FFCB_HD float2 cscale(float2 a, float s) { return __fmul2_rn(a, make_float2(s, s)); }
-#else
-FFCB_HD float2 cmul(float2 a, float2 b) { return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
 FFCB_HD float2 cadd(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
 FFCB_HD float2 csub(float2 a, float2 b) { return make_float2(a.x - b.x, a.y - b.y); }
 FFCB_HD float2 cscale(float2 a, float s) { return make_float2(a.x * s, a.y * s); }
-#endif
 
 // multiply by -i (forward transform) or +i (inverse)
 template <bool INV>

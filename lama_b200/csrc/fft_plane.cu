@@ -33,8 +33,8 @@ template <int PCH> struct PlaneCfg {
   static constexpr int ctas_per_sm = PCH == 8 ? 1 : 2;
 };
 
-// Forward: rows by the first 32*PCH threads, the 33 x PCH column tasks by the first 33*PCH (for PCH = 8 measured
-// faster than the packed 256-thread variant: 152 registers instead of 255, and one more warp to hide latency).
+// Forward: rows by the first 32*PCH threads, the 33 x PCH column tasks by the first 33*PCH (for PCH = 8 chosen
+// over the packed 256-thread variant: fewer registers per thread, and one more warp to hide latency).
 template <int PCH, int OCC>
 __global__ void __launch_bounds__(PlaneCfg<PCH>::col_threads, OCC)
 rfft2_plane64_kernel(View in, View spec, float scale) {
@@ -74,9 +74,8 @@ rfft2_plane64_kernel(View in, View spec, float scale) {
 }
 
 // Forward, second revision (default for float32 inputs).  Same algorithm and thread mapping; the differences are in
-// what surrounds the arithmetic, which is where round 1's profile put the time (profiles/r01_fft_kernels_ncu_full.txt:
-// 35% issue utilisation, `no_instruction` the top stall, a third of the 6.1 K-instruction body is 64-bit address
-// arithmetic and every access carries both format branches):
+// what surrounds the arithmetic (a third of the first revision's instruction body is 64-bit address arithmetic and
+// every access carries both format branches):
 //   * the spectrum format is a template parameter (one store path compiled in, no branch per store),
 //   * the CTA's base pointers are uniform (blockIdx-only) and every thread addresses with 32-bit offsets.
 template <int PCH, bool SPLIT>
@@ -390,8 +389,8 @@ bool inv_v2_eligible(const ffcb_tensor* spec, const ffcb_tensor* residual, const
   return vec_ok(out, out->fmt == FFCB_F32 ? 4 : 8);
 }
 
-// default: the second-revision plane kernel (measured 135 us vs 160 us for the two-pass kernels at B=32, C=192,
-// profiles/r01_fft_microbench_v2.jsonl); 0 selects the two-pass kernels, which also take every view it cannot handle
+// default: the second-revision plane kernel; 0 selects the two-pass kernels, which also take every view it cannot
+// handle
 constexpr int kDefaultInvPlaneVariant = 3;
 int inv_plane_variant() {
   const char* e = getenv("FFCB_FFT_INV_PLANE");

@@ -79,7 +79,7 @@ __global__ void fold_reflect_kernel(View gp, View add0, View add1, View out) {
 
 int grid_for(long long total) {
   const long long blocks = (total + 255) / 256;
-  return (int)(blocks < 148 * 16 ? blocks : 148 * 16);
+  return (int)(blocks < 132 * 16 ? blocks : 132 * 16);
 }
 
 }  // namespace

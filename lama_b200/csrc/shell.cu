@@ -48,8 +48,7 @@ __global__ void __launch_bounds__(kShellThreads) stem_conv7_kernel(const float* 
   }
   __syncthreads();
 
-  // accumulators as channel pairs: Blackwell issues scalar FFMA at half rate; the packed
-  // fma.rn.f32x2 (FFMA2) does two per lane per issue slot
+  // accumulators as channel pairs (ffma2: one rounding per lane)
   float2 acc[4][SN / 2];
 #pragma unroll
   for (int r = 0; r < 4; ++r)
@@ -71,7 +70,7 @@ __global__ void __launch_bounds__(kShellThreads) stem_conv7_kernel(const float* 
           const float a = prow[4 * r * PW + kx];
           const float2 aa = make_float2(a, a);
 #pragma unroll
-          for (int j = 0; j < SN / 2; ++j) acc[r][j] = __ffma2_rn(aa, wv[j], acc[r][j]);
+          for (int j = 0; j < SN / 2; ++j) acc[r][j] = ffma2(aa, wv[j], acc[r][j]);
         }
       }
     }
@@ -192,7 +191,7 @@ __global__ void __launch_bounds__(kShellThreads) head_conv7_kernel(View in, cons
   const int x0 = (blockIdx.x % tiles_x) * TX, y0 = (blockIdx.x / tiles_x) * TY;
   const int b = blockIdx.y;
 
-  // two partial sums per output (even / odd channels) so that every step is one packed FFMA2
+  // two partial sums per output (even / odd channels), accumulated as float2 pairs
   float2 acc[4][4];
 #pragma unroll
   for (int r = 0; r < 4; ++r)
@@ -228,8 +227,8 @@ __global__ void __launch_bounds__(kShellThreads) head_conv7_kernel(View in, cons
             const float2 wlo = make_float2(wv.x, wv.y), whi = make_float2(wv.z, wv.w);
 #pragma unroll
             for (int r = 0; r < 4; ++r) {
-              acc[r][n] = __ffma2_rn(make_float2(a[r + ky].x, a[r + ky].y), wlo, acc[r][n]);
-              acc[r][n] = __ffma2_rn(make_float2(a[r + ky].z, a[r + ky].w), whi, acc[r][n]);
+              acc[r][n] = ffma2(make_float2(a[r + ky].x, a[r + ky].y), wlo, acc[r][n]);
+              acc[r][n] = ffma2(make_float2(a[r + ky].z, a[r + ky].w), whi, acc[r][n]);
             }
           }
           if (N == 4) {
@@ -237,8 +236,8 @@ __global__ void __launch_bounds__(kShellThreads) head_conv7_kernel(View in, cons
             const float2 wlo = make_float2(wv.x, wv.y), whi = make_float2(wv.z, wv.w);
 #pragma unroll
             for (int r = 0; r < 4; ++r) {
-              acc[r][3] = __ffma2_rn(make_float2(a[r + ky].x, a[r + ky].y), wlo, acc[r][3]);
-              acc[r][3] = __ffma2_rn(make_float2(a[r + ky].z, a[r + ky].w), whi, acc[r][3]);
+              acc[r][3] = ffma2(make_float2(a[r + ky].x, a[r + ky].y), wlo, acc[r][3]);
+              acc[r][3] = ffma2(make_float2(a[r + ky].z, a[r + ky].w), whi, acc[r][3]);
             }
           }
         }
@@ -420,7 +419,7 @@ int stem_pack(const float* x, int B, int Cin, int H, int W, const ffcb_tensor* p
                "stem_pack: packed view must be (B, H+6, W+8, 8)");
   const long long total = (long long)B * (H + 6) * (W + 8);
   if (total == 0) return FFCB_OK;
-  const int blocks = (int)((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
+  const int blocks = (int)((total + 255) / 256 < 132 * 16 ? (total + 255) / 256 : 132 * 16);
   stem_pack_kernel<<<blocks, 256, 0, stream>>>(x, Cin, H, W, make_view(*packed));
   FFCB_LAUNCH_CHECK("stem_pack_kernel");
   return FFCB_OK;
@@ -438,7 +437,7 @@ int stem_pack_u8(const uint8_t* img, const uint8_t* mask, int B, int H0, int W0,
                "stem_pack_u8: %dx%d cannot be symmetric-padded to %dx%d", H0, W0, H, W);
   const long long total = (long long)B * (H + 6) * (W + 8);
   if (total == 0) return FFCB_OK;
-  const int blocks = (int)((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
+  const int blocks = (int)((total + 255) / 256 < 132 * 16 ? (total + 255) / 256 : 132 * 16);
   stem_pack_u8_kernel<<<blocks, 256, 0, stream>>>(img, mask, H0, W0, make_view(*packed));
   FFCB_LAUNCH_CHECK("stem_pack_u8_kernel");
   return FFCB_OK;
@@ -522,7 +521,7 @@ int fill_reflect_border(const ffcb_tensor* t, cudaStream_t stream) {
   FFCB_REQUIRE(t->H > t->pad && t->W > t->pad, "fill_reflect_border: reflect needs H,W > pad");
   const long long total = (long long)t->B * (2 * t->pad * (t->W + 2 * t->pad) + 2 * t->pad * t->H) * (t->C / 4);
   if (total == 0) return FFCB_OK;
-  const int blocks = (int)((total + 255) / 256 < 148 * 8 ? (total + 255) / 256 : 148 * 8);
+  const int blocks = (int)((total + 255) / 256 < 132 * 8 ? (total + 255) / 256 : 132 * 8);
   reflect_ring_kernel<<<blocks, 256, 0, stream>>>(make_view(*t));
   FFCB_LAUNCH_CHECK("reflect_ring_kernel");
   return FFCB_OK;

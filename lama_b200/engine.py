@@ -28,7 +28,7 @@ from . import _lib as L
 from . import packing as P
 
 PROGRAM_CACHE_SIZE = 3          # executors (programs + their buffers) kept per module, LRU
-MATH_ENV = "LAMA_B200_MATH"     # "bf16x3" (default: tcgen05 arm) | "fp32" (CUDA-core arm)
+MATH_ENV = "LAMA_B200_MATH"     # "bf16x3" (default: wgmma arm) | "fp32" (CUDA-core arm)
 
 
 def default_math() -> int:
@@ -48,7 +48,7 @@ class Buf:
     fmt: int = L.F32
     reflect_border: int = 0
     cg: int = 0        # > 0: channel-group planar storage [C/cg][B][H][W][cg] (FourierUnit chain, include/ffc_b200.h)
-    tile: int = 0      # 128 (with cg == 8, split bf16): tile-blocked [pixel block of 128][C/8][128][8] — tcgen05 operand tiles
+    tile: int = 0      # 128 (with cg == 8, split bf16): tile-blocked [pixel block of 128][C/8][128][8] — wgmma operand tiles
 
 
 @dataclass
@@ -448,9 +448,7 @@ def _fold(bn, n, device):
 
 def fu_batch_chunk(batch: int, h: int, w: int, c: int) -> int:
     """Images per pass of the rfft2 -> GEMM -> irfft2 chain.  Running the chain over slices of the batch keeps
-    its intermediates inside the 126 MB L2, but measured on B200 (bs32, 512x512: 624 img/s unsliced vs 600-620
-    with 6..16-image slices, profiles/r01_fu_chunk_sweep.txt) the extra launches and partial waves cost more than
-    the L2 hits save — the kernels are latency- not bandwidth-bound.  Default: whole batch;
+    its intermediates inside the 50 MB L2 at the cost of extra launches and partial waves.  Default: whole batch;
     LAMA_B200_FU_CHUNK=n slices."""
     n = int(os.environ.get("LAMA_B200_FU_CHUNK", "0"))
     return batch if n <= 0 else min(batch, n)
@@ -459,7 +457,7 @@ def fu_batch_chunk(batch: int, h: int, w: int, c: int) -> int:
 def fu_planar_ok(prog: Program, st, h: int, w: int) -> bool:
     """Channel-group planar storage for the SpectralTransform chain (conv1 -> rfft2 -> spectral conv -> irfft2 ->
     conv2): every (image, 4-channel group) plane set is one dense block for the second-generation plane FFT kernels
-    (csrc/fft_plane_cg.cu) and the GEMMs read [K/8][pixel][8] operand tiles.  Needs the tcgen05 arm, 64x64 or 32x32
+    (csrc/fft_plane_cg.cu) and the GEMMs read [K/8][pixel][8] operand tiles.  Needs the tensor-core arm, 64x64 or 32x32
     planes (the 512x512 / 256x256 bottleneck) and whole 64-channel K blocks on every contraction of the chain.
     LAMA_B200_FU_LAYOUT=nhwc keeps the round-1 channels-last chain (A/B measurements)."""
     if prog.math != L.MATH_BF16X3 or os.environ.get("LAMA_B200_FU_LAYOUT", "planar") != "planar":
@@ -481,7 +479,7 @@ _PLANAR_OK: Dict[int, bool] = {}
 def planar_selftest(device: torch.device) -> bool:
     """Once per process and device: run the planar chain's three kernels (plane FFT pair, interleaved-operand GEMM with
     a planar output) on a small random problem and compare with torch on the same device.  The chain depends on
-    details no compile-time check covers (tcgen05 no-swizzle descriptor fields, bulk-copy tile layout); if the check
+    details no compile-time check covers (wgmma no-swizzle descriptor fields, bulk-copy tile layout); if the check
     fails the process keeps the channels-last chain of round 1 (still the native kernels) and says so loudly —
     LAMA_B200_FU_LAYOUT=planar! skips the check and forces the planar chain, =nhwc forces the other."""
     idx = device.index if device.index is not None else torch.cuda.current_device()
@@ -699,7 +697,7 @@ def emit_resnet_block(prog: Program, blk, X: Buf, cl: int, cg: int, in_place: bo
 
 # Largest plane side the forward+backward block program is used for.  Hardware-validated against autograd: 32x32 and
 # 64x64 (planar chain), 12x20 and 17x25 (general FFT kernels) — tests/test_gpu_parity.py.  A late check of round 2
-# (tools/grad_check.py, profiles/r02_grad_check.json) found the program's FORWARD off by 8-14 % (2-norm) on 128-wide
+# (tools/grad_check.py) found the program's FORWARD off by 8-14 % (2-norm) on 128-wide
 # planes (128x128 and 96x128 alike, so an x-direction effect) although the CPU interpretation of the very same program
 # matches the oracle to 2e-7 and the whole-generator program is right at 128x128 and 256x256 planes: a kernel-level
 # defect specific to the standalone block program's buffers at that width, not yet located.  Until it is, planes wider
@@ -953,7 +951,7 @@ def build_generator_program(prog: Program, gen, shape, u8_size: Optional[Tuple[i
 
 
 def tc_compatible(prog: Program) -> bool:
-    """The tcgen05 arm needs 16-byte aligned bf16 pixels/slices: channel counts and slice starts in
+    """The tensor-core arm needs 16-byte aligned bf16 pixels/slices: channel counts and slice starts in
     multiples of 8.  Programs that do not qualify run the fp32 CUDA-core arm (still native)."""
     for op in prog.ops:
         if isinstance(op, ConvOp):
@@ -968,7 +966,7 @@ def tc_compatible(prog: Program) -> bool:
 
 
 def insert_border_ops(prog: Program):
-    """Producers never write the reflected ring of a padded buffer (the tcgen05 epilogue stores through a
+    """Producers never write the reflected ring of a padded buffer (the tensor-core epilogue stores through a
     tensor map of the interior; layout conversions, the stem and the FFT kernels write pixels only).  Insert
     a BorderOp lazily: right before the first contraction that reads a buffer whose interior changed since
     its ring was last rebuilt.  For the in-place residual blocks that is one ring refresh per FFC_BN_ACT."""
@@ -991,7 +989,7 @@ def insert_border_ops(prog: Program):
 
 
 def conv_writes_ring(prog: Program, op) -> bool:
-    """The tcgen05 contraction writes the mirrored copies of rows 1 / H-2 and columns 1 / W-2 into a 1-pixel reflected
+    """The tensor-core contraction writes the mirrored copies of rows 1 / H-2 and columns 1 / W-2 into a 1-pixel reflected
     ring of its output itself (conv_tc.cu, TcParams::ring) — whole-plane outputs only (a sub-pixel phase or a window
     does not own the ring)."""
     if os.environ.get("LAMA_B200_RING_KERNEL", "0") == "1":        # A/B: always refresh rings with the ring kernel
@@ -1038,7 +1036,7 @@ def assign_storage_slots(prog: Program) -> Dict[str, int]:
     (``storage_key``) share a slot: whatever a kernel leaves unwritten (zero-initialised pixel / channel padding, the
     reflected ring before its producer ran) then holds what the same kind of buffer held there before, never foreign
     bits.  For big-lama this folds the 18 residual blocks' ~150 buffers onto two blocks' worth: 28 GB -> 10 GB at bs32
-    512x512, and bs64 1024x1024 (BASELINE config 4 on one GPU) fits a 180 GB B200 at all.  Constant buffers
+    512x512, and bs64 1024x1024 (BASELINE config 4's global batch) pools to about 64 GB.  Constant buffers
     (``prog.consts``) keep their own storage; ``LAMA_B200_POOL=0`` gives every buffer its own."""
     first: Dict[str, int] = {}
     last: Dict[str, int] = {}

@@ -6,7 +6,7 @@ a silent mismatch would go unnoticed) and forward conventions (FFC-family module
 ``(x_l, x_g)`` tuples whose empty side is the int ``0``, ffc.py:206,225).
 
 Execution: on a CUDA tensor, in ``eval()`` mode with autograd off and float32 input, every module
-runs the hand-written sm_100a kernels of ``libffc_b200.so`` through a cached *program*
+runs the hand-written sm_90a kernels of ``libffc_b200.so`` through a cached *program*
 (``lama_b200.engine``).  Options no shipped config enables (LFU, gating, SE, positional encoding,
 3-D FFT, spatial rescaling, groups, non-ortho norm, non-BatchNorm norms, dilation != 1,
 spatial-transform wrappers) and training/autograd run the same maths as a composition of torch

@@ -1,5 +1,5 @@
 """``torch.library`` registration of the native generator call, so that a ``torch.jit.trace`` of the drop-in model
-(the reference's ``bin/to_jit.py:49-60``) KEEPS the sm_100a kernels instead of silently baking in cuFFT / cuDNN.
+(the reference's ``bin/to_jit.py:49-60``) KEEPS the sm_90a kernels instead of silently baking in cuFFT / cuDNN.
 
 A ctypes call is invisible to the tracer.  The op below makes the whole generator one node of the traced graph:
 

@@ -57,7 +57,7 @@ class PackedConv:
 
     def split_weights(self) -> torch.Tensor:
         """bf16 [2][N][Kpad]: K-major, every segment zero-padded to a multiple of 64 channels (one
-        128-byte swizzle row per K block of the tcgen05 arm)."""
+        128-byte swizzle row per K block of the wgmma arm)."""
         if self.w_split is None:
             w_nk = self.w_kn.t()
             cols, k0 = [], 0

@@ -189,7 +189,7 @@ def predict_directory(inpainter: BatchedInpainter, indir: str, outdir: str, img_
 
 
 def main(argv=None):
-    ap = argparse.ArgumentParser(description="batched LaMa inpainting on the native B200 path")
+    ap = argparse.ArgumentParser(description="batched LaMa inpainting on the native H100 path")
     ap.add_argument("--model-dir", required=True, help="directory with config.yaml and models/<checkpoint>")
     ap.add_argument("--checkpoint", default="best.ckpt")
     ap.add_argument("--indir", required=True)

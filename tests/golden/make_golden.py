@@ -222,12 +222,39 @@ def make_f4():
     _save("resblock_64_lfu_8x8", x_l=xl.numpy(), x_g=xg.numpy(), y_l=yl.numpy(), y_g=yg.numpy(), **_sd_np(m))
 
 
+@torch.no_grad()
+def make_surface():
+    """Module surface outside the generator: an FFC_BN_ACT with LFU on CPU tensors (the torch-composition path of
+    the drop-in) and the training-only FFCNLayerDiscriminator.  The state_dict is stored whole (num_batches_tracked
+    included) so that the drop-in can load it with strict=True."""
+    ffc = load_reference_ffc()
+    torch.set_num_threads(1)
+    kw = dict(in_channels=32, out_channels=32, kernel_size=3, ratio_gin=0.75, ratio_gout=0.75, padding=1,
+              activation_layer=torch.nn.ReLU, enable_lfu=True)
+    m = seeded_parameters_(ffc.FFC_BN_ACT(**kw).eval(), 5)
+    xl, xg = _randn((1, 8, 8, 8), 800), _randn((1, 24, 8, 8), 801)
+    yl, yg = m((xl, xg))
+    sd = {"sd::" + k: v.numpy() for k, v in m.state_dict().items()}
+    _save("ffcbnact_32_lfu_cpu_8x8", x_l=xl.numpy(), x_g=xg.numpy(), y_l=yl.numpy(), y_g=yg.numpy(), **sd)
+    kw = dict(input_nc=3, ndf=16, n_layers=3, init_conv_kwargs=dict(ratio_gin=0, ratio_gout=0.5, enable_lfu=False),
+              conv_kwargs=dict(ratio_gin=0.5, ratio_gout=0.5, enable_lfu=False))
+    m = seeded_parameters_(ffc.FFCNLayerDiscriminator(**kw).eval(), 9)
+    x = torch.randn(1, 3, 32, 32, generator=torch.Generator().manual_seed(1))
+    y, feats = m(x)
+    sd = {"sd::" + k: v.numpy() for k, v in m.state_dict().items()}
+    _save("discriminator_ndf16_32x32", x=x.numpy(), y=y.numpy(), **{"feat%d" % i: t.numpy() for i, t in enumerate(feats)},
+          **sd)
+
+
 if __name__ == "__main__":
     if "--f4-only" in sys.argv:
         make_f4()
     elif "--predict-only" in sys.argv:
         make_predict()
+    elif "--surface-only" in sys.argv:
+        make_surface()
     else:
         main()
         make_predict()
         make_f4()
+        make_surface()

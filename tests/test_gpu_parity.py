@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box: ``pytest -m gpu``).  Everything goes through the C ABI of
+"""GPU parity tests (run on an H100: ``pytest -m gpu``).  Everything goes through the C ABI of
 libffc_b200.so (via the drop-in modules / lama_b200.engine); the checker is the oracle
 (oracle/ffc_numpy.py float64, oracle/ffc_torch_cpu.py) and the committed goldens generated from the
 unmodified reference.  /root/reference is NOT read here.
@@ -212,7 +212,7 @@ def test_fft_round_trip_full_size():
 
 # ------------------------------------------------------------------------------------ conv kernel
 _CONV_CASES = ["k3_reflect", "k3_s2", "k1_two_src", "k7_nopad", "zero_border_phase", "ragged"]
-# (the tcgen05 arm requires 64-channel K segments: "k7_nopad" and "ragged" exist for the CUDA-core arm only)
+# (the tensor-core arm requires 64-channel K segments: "k7_nopad" and "ragged" exist for the CUDA-core arm only)
 _CONV_PARAMS = [(c, m) for m in MATHS for c in _CONV_CASES
                 if not (m == L.MATH_BF16X3 and c in ("k7_nopad", "ragged"))]
 

@@ -75,39 +75,38 @@ def test_state_dict_schema_matches_reference():
     assert isinstance(g.model, torch.nn.Sequential) and len(g.model) == 36
 
 
+def _golden_module(name):
+    """(arrays, state_dict as tensors) of a fixture made from the reference by tests/golden/make_golden.py."""
+    z = np.load(os.path.join(ROOT, "tests", "golden", name + ".npz"))
+    return ({k: torch.from_numpy(z[k]) for k in z.files if not k.startswith("sd::")},
+            {k[4:]: torch.from_numpy(z[k]) for k in z.files if k.startswith("sd::")})
+
+
 def test_module_torch_composition_matches_reference_on_cpu():
-    """Feature-fallback path (CPU tensors / unsupported options) is the reference's operator sequence."""
-    from oracle import ref_import
-    if not ref_import.available():
-        pytest.skip("reference tree not present")
-    ffc = ref_import.load_reference_ffc()
+    """Feature-fallback path (CPU tensors / unsupported options) is the reference's operator sequence: an LFU
+    FFC_BN_ACT against the reference's outputs stored in tests/golden/ffcbnact_32_lfu_cpu_8x8.npz."""
     kw = dict(in_channels=32, out_channels=32, kernel_size=3, ratio_gin=0.75, ratio_gout=0.75, padding=1,
               activation_layer=torch.nn.ReLU, enable_lfu=True)
-    ref = seeded_parameters_(ffc.FFC_BN_ACT(**kw).eval(), 5)
+    a, sd = _golden_module("ffcbnact_32_lfu_cpu_8x8")
     ours = M.FFC_BN_ACT(**kw).eval()
-    ours.load_state_dict(ref.state_dict(), strict=True)
-    xl, xg = torch.randn(1, 8, 8, 8), torch.randn(1, 24, 8, 8)
+    ours.load_state_dict(sd, strict=True)
     with torch.no_grad():
-        a, b = ref((xl, xg)); c, d = ours((xl, xg))
-    assert torch.allclose(a, c, atol=1e-6) and torch.allclose(b, d, atol=1e-6)
+        c, d = ours((a["x_l"], a["x_g"]))
+    assert torch.allclose(a["y_l"], c, atol=1e-6) and torch.allclose(a["y_g"], d, atol=1e-6)
 
 
 def test_discriminator_surface_matches_reference():
-    """FFCNLayerDiscriminator (ffc.py:370-433, training only) keeps the reference's state_dict and outputs."""
-    from oracle import ref_import
-    if not ref_import.available():
-        pytest.skip("reference tree not present")
-    ffc = ref_import.load_reference_ffc()
+    """FFCNLayerDiscriminator (ffc.py:370-433, training only) keeps the reference's state_dict and outputs (stored in
+    tests/golden/discriminator_ndf16_32x32.npz)."""
     kw = dict(input_nc=3, ndf=16, n_layers=3, init_conv_kwargs=dict(ratio_gin=0, ratio_gout=0.5, enable_lfu=False),
               conv_kwargs=dict(ratio_gin=0.5, ratio_gout=0.5, enable_lfu=False))
-    ref = seeded_parameters_(ffc.FFCNLayerDiscriminator(**kw).eval(), 9)
+    a, sd = _golden_module("discriminator_ndf16_32x32")
     ours = M.FFCNLayerDiscriminator(**kw).eval()
-    ours.load_state_dict(ref.state_dict(), strict=True)
-    x = torch.randn(1, 3, 32, 32, generator=torch.Generator().manual_seed(1))
+    ours.load_state_dict(sd, strict=True)
     with torch.no_grad():
-        a, fa = ref(x)
-        b, fb = ours(x)
-    assert torch.allclose(a, b, atol=1e-6) and len(fa) == len(fb)
+        b, fb = ours(a["x"])
+    fa = [a["feat%d" % i] for i in range(sum(k.startswith("feat") for k in a))]
+    assert torch.allclose(a["y"], b, atol=1e-6) and len(fa) == len(fb)
     assert all(torch.allclose(p, q, atol=1e-6) for p, q in zip(fa, fb))
 
 

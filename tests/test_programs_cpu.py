@@ -198,7 +198,7 @@ def test_bf16x3_program_layout_and_semantics():
     assert isinstance(ops[0], E.StemPackOp) and isinstance(ops[1], E.ConvOp) and isinstance(ops[2], E.ConvOp)
     assert ops[1].ins[0].window == 8 and len(ops[1].packed.segs) == 4        # two-row packing: kernel rows (0,1) (2,3) (4,5) (6,-)
     # ring discipline: whenever a contraction reads a ring buffer, every op that touched that buffer since the ring
-    # was last complete either was a BorderOp or a whole-plane tcgen05 contraction (its epilogue writes the mirrored
+    # was last complete either was a BorderOp or a whole-plane tensor-core contraction (its epilogue writes the mirrored
     # pixels itself: engine.conv_writes_ring), and no BorderOp is redundant.
     last = {}
     for o in ops:
@@ -220,7 +220,7 @@ def test_bf16x3_program_layout_and_semantics():
     assert n_border == 3      # only the 3 up-sampled outputs (written as sub-pixel phases) need the ring kernel
     out = SpecInterpreter(prog).run({"x0": x})
     assert float(np.abs(out["y0"].numpy() - a["y"]).max()) < 2e-6
-    # weights of the tcgen05 arm: [2][N][Kpad], K padded per segment to 64
+    # weights of the tensor-core arm: [2][N][Kpad], K padded per segment to 64
     conv = next(o for o in ops if isinstance(o, E.ConvOp))
     ws = conv.packed.split_weights()
     assert ws.dtype == torch.bfloat16 and ws.shape[0] == 2 and ws.shape[2] == 64 * len(conv.packed.segs)
@@ -360,7 +360,7 @@ def test_empty_batch_returns_empty_outputs_without_launching():
 def test_storage_slots_never_alias_live_buffers(monkeypatch):
     """engine.assign_storage_slots: buffers share storage only when (a) their storage is byte-identical and (b) the
     last op touching the earlier one comes strictly before the first op touching the later one; constants keep their
-    own storage.  big-lama folds onto a dozen slots (bs64 1024x1024 = BASELINE config 4 on one GPU must fit 180 GB)."""
+    own storage.  big-lama folds onto a dozen slots (bs64 1024x1024 = BASELINE config 4's global batch pools under 80 GB)."""
     from lama_b200.testing import BIG_LAMA_KWARGS
     gen = M.FFCResNetGenerator(**BIG_LAMA_KWARGS).eval()
     with torch.no_grad():

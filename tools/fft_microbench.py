@@ -103,14 +103,7 @@ if __name__ == "__main__":
             for flush_mb in (0, 512):
                 print(json.dumps(time_fu_chain(*fu, planar, flush_mb=flush_mb)), flush=True)
         sys.exit(0)
-    if "--gemm-knobs" in sys.argv:       # where does the planar spectral GEMM spend its time? (FFCB_TC_DEBUG stage skipping)
-        for lanes in ("32", "1"):
-            for dbg in ("0", "1", "2", "8", "10"):
-                os.environ["FFCB_TC_DEBUG"] = dbg
-                os.environ["FFCB_TC_BULK_LANES"] = lanes
-                r = time_fu_chain(*fu, True, reps=10)
-                print(json.dumps({"bulk_lanes": lanes, "FFCB_TC_DEBUG": dbg, "gemm_us": r["gemm_us"]}), flush=True)
-        os.environ.pop("FFCB_TC_DEBUG"); os.environ.pop("FFCB_TC_BULK_LANES")
+    if "--l2-hints" in sys.argv:         # planar chain with and without the L2 residency hints
         for hints in ("1", "0"):
             os.environ["FFCB_L2_HINTS"] = hints
             print(json.dumps({"FFCB_L2_HINTS": hints, **time_fu_chain(*fu, True, reps=10)}), flush=True)
