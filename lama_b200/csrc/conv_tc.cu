@@ -22,8 +22,10 @@
 // before, and after the last K block runs the epilogue from its registers (shift / addend / activation -> split-bf16
 // or fp32 channels-last stores, or planar float32 stores; the reflected ring of a whole-plane output is written here
 // too).  The producer runs up to `stages` K blocks ahead, so the loads of the next tile overlap the epilogue.
-// Template parameters select the operand / output kinds (IL, PO) and the rows-resident mode of the 7x7 shell layers
-// (RR: one halo load per M tile, resident weight tiles).
+// Template parameters select the operand / output kinds (IL, PO), the rows-resident mode of the 7x7 shell layers
+// (RR: one halo load per M tile, resident weight tiles) and the column-halo mode of stride-1 3x3 contractions (HALO:
+// per M tile, 64-channel block and column shift one box serves the three taps of that column; see
+// TcParams::seg_taps).
 #include <cuda.h>
 #include <stdlib.h>
 
@@ -73,6 +75,17 @@ struct TcParams {
   // (dy - dy0) * TW rows further down) and the (small) weight tiles of all segments stay resident in shared memory
   // for the whole kernel.
   int rr_dy0, rr_a_bytes, rr_w_bytes;
+  // Column-halo mode (template HALO; stride-1 3x3 reflect contractions over ring-padded channels-last sources, 64 x 2
+  // tiles).  The K order is channel-block-major, then dx, then dy: per M tile, 64-channel block of a complete 3x3 group
+  // (nine consecutive segments, same src / c0 / nch, every (dy,dx) in {-1,0,1}^2) and column shift dx, ONE TMA box of
+  // (64 ch, TW, TH+2) pixels per plane lands in an A buffer, and the three taps of that column read it dy * TW rows
+  // further down — whole 1024-byte swizzle atoms, as in RR — so 3 boxes of 4 rows replace 9 boxes of 2 rows (a third
+  // fewer activation bytes into shared memory).  Every other segment is a one-tap group over the same kind of box.
+  // Shared memory: 2 A buffers x (hi | lo) x halo_a_bytes (2 x 2 x 32 KB at 64 x 2), then a ring of one-tap weight
+  // stages: 64 channels x BN x (hi | lo) = 32 KB at BN = 128, 3 of them in 227 KB.
+  // seg_taps[s]: 9 = segment s starts a 3x3 group, 0 = inside one, 1 = a one-tap group.
+  int halo_a_bytes;
+  signed char seg_taps[FFCB_MAX_KSEG];
   ffcb_kseg seg[FFCB_MAX_KSEG];
 };
 
@@ -263,21 +276,26 @@ __device__ __forceinline__ TileCoord tile_coord(const TcParams& p, long long m_t
 // whole contraction with one descriptor kind.
 // PO: the output is channel-group planar float32.
 // BN: the N tile (TcParams::BN), a compile-time wgmma shape.
-template <bool IL, bool PO, bool RR, int BN>
+template <bool IL, bool PO, bool RR, bool HALO, int BN>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_tc_kernel(const __grid_constant__ TcParams p, const __grid_constant__ CUtensorMap map_in0,
                const __grid_constant__ CUtensorMap map_in1, const __grid_constant__ CUtensorMap map_w) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve: [RR: resident weights] stages of [A_hi | A_lo | W_hi | W_lo], then barriers
+  // carve: [RR: resident weights | HALO: 2 A buffers of (hi | lo)] stages of [A_hi | A_lo | W_hi | W_lo] (HALO: one-tap
+  // weight stages [W_hi | W_lo]), then barriers
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const int w_bytes = p.BN * BK * 2;
-  const int stage_bytes = RR ? 2 * p.rr_a_bytes : 2 * kTileABytes + 2 * w_bytes;
+  const int stage_bytes = RR ? 2 * p.rr_a_bytes : HALO ? 2 * w_bytes : 2 * kTileABytes + 2 * w_bytes;
   uint8_t* w_res = smem;                                   // RR: resident weight tiles [seg][hi | lo]
+  uint8_t* a_buf = smem;                                   // HALO: A buffers [2][hi | lo]
   if constexpr (RR) smem += p.rr_w_bytes;
+  if constexpr (HALO) smem += (size_t)4 * p.halo_a_bytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * stage_bytes);
   uint64_t* full = bars;
   uint64_t* empty = bars + kMaxStages;
   uint64_t* w_bar = bars + 2 * kMaxStages;                 // RR: the resident weights have landed
+  uint64_t* a_full = bars + 2 * kMaxStages + 1;            // HALO: A buffer landed / released (2 each)
+  uint64_t* a_empty = a_full + 2;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
@@ -289,6 +307,8 @@ conv_tc_kernel(const __grid_constant__ TcParams p, const __grid_constant__ CUten
   if (warp == 1 && lane == 0) {
     for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kConsumers); }
     if constexpr (RR) mbar_init(w_bar, 1);
+    if constexpr (HALO)
+      for (int s = 0; s < 2; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], kConsumers); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -300,7 +320,54 @@ conv_tc_kernel(const __grid_constant__ TcParams p, const __grid_constant__ CUten
 
   if (warp == 0) {
     // ================================================================ TMA producer (uniform control flow, one elected lane issues)
-    if constexpr (RR) {
+    if constexpr (HALO) {
+      // per group, 64-channel block and column shift dx: the A buffer (the column box shifted by dx), then one weight
+      // stage per tap of that column (weight K of tap t, block j = kofs + (t * nblk + j) * 64, kofs = the group's
+      // first K)
+      int stage = 0, ast = 0;
+      uint32_t phase = 0, aph = 0;
+      for (long long t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+        const int n_tile = (int)(t % p.num_n_tiles);
+        const TileCoord tc = tile_coord(p, t / p.num_n_tiles);
+        int kofs = 0;
+        for (int s = 0; s < p.nseg;) {
+          const int ntap = p.seg_taps[s];
+          const ffcb_kseg g = p.seg[s];
+          const CUtensorMap* map = g.src ? &map_in1 : &map_in0;
+          const int nblk = (g.nch + BK - 1) / BK;
+          for (int j = 0; j < nblk; ++j) {
+            for (int u = 0; u < (ntap == 9 ? 3 : 1); ++u) {
+              const int dxu = ntap == 9 ? u - 1 : g.dx;
+              mbar_wait(&a_empty[ast], aph ^ 1);
+              if (elect_one()) {
+                uint8_t* ab = a_buf + (size_t)ast * 2 * p.halo_a_bytes;
+                mbar_expect_tx(&a_full[ast], 2u * p.TW * (p.TH + 2) * BK * 2);
+                const int cx = tc.x0 + dxu + p.coord_off[g.src], cy = tc.y0 - 1 + p.coord_off[g.src];
+                tma_load_5d(ab, map, &a_full[ast], g.c0 + j * BK, cx, cy, tc.b, 0);
+                tma_load_5d(ab + p.halo_a_bytes, map, &a_full[ast], g.c0 + j * BK, cx, cy, tc.b, 1);
+              }
+              __syncwarp();
+              if (++ast == 2) { ast = 0; aph ^= 1; }
+              for (int tap = 0; tap < ntap; ++tap) {
+                if (p.seg[s + tap].dx != dxu) continue;
+                mbar_wait(&empty[stage], phase ^ 1);
+                if (elect_one()) {
+                  uint8_t* st = smem + (size_t)stage * stage_bytes;
+                  mbar_expect_tx(&full[stage], (uint32_t)stage_bytes);
+                  const int k = kofs + (tap * nblk + j) * BK;
+                  tma_load_3d(st, &map_w, &full[stage], k, n_tile * p.BN, 0);
+                  tma_load_3d(st + w_bytes, &map_w, &full[stage], k, n_tile * p.BN, 1);
+                }
+                __syncwarp();
+                if (++stage == p.stages) { stage = 0; phase ^= 1; }
+              }
+            }
+          }
+          kofs += ntap * nblk * BK;
+          s += ntap;
+        }
+      }
+    } else if constexpr (RR) {
       const ffcb_kseg g0 = p.seg[0];
       const CUtensorMap* map = g0.src ? &map_in1 : &map_in0;
       if (elect_one()) {
@@ -387,14 +454,68 @@ conv_tc_kernel(const __grid_constant__ TcParams p, const __grid_constant__ CUten
     float acc[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-    int stage = 0;
-    uint32_t phase = 0;
+    int stage = 0, ast = 0;
+    uint32_t phase = 0, aph = 0;
+    // HALO: row of the column box holding this warpgroup's first pixel at dy = 0 (tile row g, below the top halo row)
+    const int a_row0 = (g + 1) * p.TW;
     if constexpr (RR) mbar_wait(w_bar, 0);
     for (long long t = blockIdx.x; t < num_tiles; t += gridDim.x) {
       const int n_tile = (int)(t % p.num_n_tiles);
       const TileCoord tc = tile_coord(p, t / p.num_n_tiles);
       fence_acc<BN>(acc);
-      if constexpr (RR) {
+      if constexpr (HALO) {
+        // Release protocol (one tap of wgmmas in flight, wait<1>).  A weight stage goes back after the wait of the next
+        // tap: its wgmmas have retired then.  An A buffer is read by every tap of its column, so it goes back only
+        // after the wait of the FIRST tap of the next column, which retires the column's last wgmmas.  The end of the
+        // tile (wait<0>) releases the last of each.
+        int prev = -1, a_prev = -1, nt = 0;
+        for (int s = 0; s < p.nseg;) {
+          const int ntap = p.seg_taps[s];
+          const int nblk = (p.seg[s].nch + BK - 1) / BK;
+          for (int j = 0; j < nblk; ++j) {
+            for (int u = 0; u < (ntap == 9 ? 3 : 1); ++u) {
+              const int dxu = ntap == 9 ? u - 1 : p.seg[s].dx;
+              mbar_wait(&a_full[ast], aph);
+              const uint32_t ab = smem_u32(a_buf + (size_t)ast * 2 * p.halo_a_bytes);
+              for (int tap = 0; tap < ntap; ++tap) {
+                const int dy = p.seg[s + tap].dy;
+                if (p.seg[s + tap].dx != dxu) continue;
+                // this warpgroup's 64 pixels shifted by dy: 64 rows of 128 B further down per row of the column box,
+                // whole 1024-byte swizzle atoms
+                const uint32_t a_off = (uint32_t)((a_row0 + dy * p.TW) * (BK * 2)) >> 4;
+                const uint32_t a_hi = desc_addr(ab) + a_off;
+                const uint32_t a_lo = desc_addr(ab + (uint32_t)p.halo_a_bytes) + a_off;
+                mbar_wait(&full[stage], phase);
+                wgmma_fence();
+                const uint32_t st = smem_u32(smem + (size_t)stage * stage_bytes);
+                const uint32_t w_hi = desc_addr(st), w_lo = desc_addr(st + (uint32_t)w_bytes);
+#pragma unroll
+                for (int k = 0; k < BK / WG_K; ++k) {
+                  const uint32_t adv = (uint32_t)((k * WG_K * 2) >> 4);     // +32 B per K = 16 inside the swizzle row
+                  wgmma_bn<BN>(acc, desc64((a_hi + adv) | kLoSw, kHiSw), desc64((w_hi + adv) | kLoSw, kHiSw),
+                               (nt | k) != 0);
+                  wgmma_bn<BN>(acc, desc64((a_lo + adv) | kLoSw, kHiSw), desc64((w_hi + adv) | kLoSw, kHiSw), 1);
+                  wgmma_bn<BN>(acc, desc64((a_hi + adv) | kLoSw, kHiSw), desc64((w_lo + adv) | kLoSw, kHiSw), 1);
+                }
+                wgmma_commit();
+                wgmma_wait<1>();
+                if (prev >= 0) mbar_arrive(&empty[prev]);
+                prev = stage;
+                if (++stage == p.stages) { stage = 0; phase ^= 1; }
+                if (a_prev >= 0) { mbar_arrive(&a_empty[a_prev]); a_prev = -1; }
+                ++nt;
+              }
+              a_prev = ast;
+              if (++ast == 2) { ast = 0; aph ^= 1; }
+            }
+          }
+          s += ntap;
+        }
+        wgmma_wait<0>();
+        fence_acc<BN>(acc);
+        mbar_arrive(&empty[prev]);
+        mbar_arrive(&a_empty[a_prev]);
+      } else if constexpr (RR) {
         mbar_wait(&full[stage], phase);
         const uint32_t st = smem_u32(smem + (size_t)stage * stage_bytes);
         const uint32_t wr = smem_u32(w_res);
@@ -677,6 +798,36 @@ int conv_tc(const ffcb_conv_desc* d, cudaStream_t stream) {
     }
     rr = rr && (rr_dy_max - rr_dy_min) <= 8;
   }
+  // column-halo mode (TcParams::seg_taps): spatial, stride 1, planes wider than 32 (the current tiling's TW >= 64),
+  // and channels-last outputs; every segment reads a reflect-ring-padded channels-last source within one pixel
+  // (coord_off >= 1); at least one complete 3x3 group.  Contractions with a tile-blocked segment (the global one:
+  // convl2g + st.conv2) keep the per-tap path: each of its one-tap groups would wait for an A buffer to turn over
+  // (DESIGN.md §9).
+  bool halo = !flat && !rr && d->stride == 1 && W > 32 && d->out.cg == 0;
+  int ngroups = 0;
+  for (int i = 0; i < d->nseg && halo;) {
+    const ffcb_kseg& g = d->seg[i];
+    const ffcb_tensor& t = d->in[g.src];
+    halo = t.cg == 0 && d->border == FFCB_BORDER_REFLECT && taps[g.src] && t.pad >= 1 && t.window == 0;
+    unsigned mask = 0;
+    int n = 0;
+    for (; n < 9 && i + n < d->nseg; ++n) {
+      const ffcb_kseg& q = d->seg[i + n];
+      if (q.src != g.src || q.c0 != g.c0 || q.nch != g.nch || q.dy < -1 || q.dy > 1 || q.dx < -1 || q.dx > 1) break;
+      mask |= 1u << ((q.dy + 1) * 3 + q.dx + 1);
+    }
+    if (n == 9 && mask == 0x1FFu) {
+      p.seg_taps[i] = 9;
+      for (int k = 1; k < 9; ++k) p.seg_taps[i + k] = 0;
+      i += 9;
+      ++ngroups;
+    } else {
+      halo = halo && g.dy >= -1 && g.dy <= 1 && g.dx >= -1 && g.dx <= 1;
+      p.seg_taps[i++] = 1;
+    }
+  }
+  halo = halo && ngroups > 0;
+  p.halo_a_bytes = 0;
   if (flat) {
     p.TW = BM; p.TH = 1; p.tiles_x = p.tiles_y = 1;
     p.num_m_tiles = ((long long)d->out.B * H * W + BM - 1) / BM;
@@ -692,6 +843,15 @@ int conv_tc(const ffcb_conv_desc* d, cudaStream_t stream) {
     p.rr_dy0 = rr_dy_min;
     p.rr_a_bytes = (p.TH + rr_dy_max - rr_dy_min) * p.TW * BK * 2;
     p.rr_w_bytes = d->nseg * 2 * p.BN * BK * 2;
+  } else if (halo) {
+    // 64 x 2 tiles for every plane width (column tiles beyond 64): each warpgroup's 64 pixels are one image row of the
+    // column box, so a dy shift is 64 rows = 8 swizzle atoms; the box is 4 x 64 pixel rows (32 KB per plane; a 128 x 1
+    // tile would need 3 x 128 rows, and two A buffers of those leave no room for weight stages)
+    p.TW = 64; p.TH = 2;
+    p.tiles_x = (W + p.TW - 1) / p.TW;
+    p.tiles_y = (H + p.TH - 1) / p.TH;
+    p.num_m_tiles = (long long)d->out.B * p.tiles_x * p.tiles_y;
+    p.halo_a_bytes = p.TW * (p.TH + 2) * BK * 2;
   } else {
     int tw = 1;
     while (tw < W && tw < BM) tw <<= 1;      // smallest power of two >= W, capped at 128
@@ -732,6 +892,7 @@ int conv_tc(const ffcb_conv_desc* d, cudaStream_t stream) {
                            (cuuint64_t)t.lo_off * esz};
       cuuint32_t box[5] = {BK, (cuuint32_t)(p.TW * d->stride), (cuuint32_t)(p.TH * d->stride), 1, 1};
       if (rr) box[2] = (cuuint32_t)(p.TH + rr_dy_max - rr_dy_min);      // the whole halo of the tile in one box
+      if (halo) box[2] = (cuuint32_t)(p.TH + 2);                         // the tile's rows and one above / below
       cuuint32_t es[5] = {1, (cuuint32_t)d->stride, (cuuint32_t)d->stride, 1, 1};
       p.coord_off[s] = off;
       if ((rc = encode(&maps[s], base, 5, dims, str, box, es, "spatial activations"))) return rc;
@@ -756,8 +917,10 @@ int conv_tc(const ffcb_conv_desc* d, cudaStream_t stream) {
   }
 
   // ---- launch
-  const int stage_bytes = rr ? 2 * p.rr_a_bytes : 2 * kTileABytes + 2 * p.BN * BK * 2;
-  const int bar_bytes = kBarBytes + (rr ? p.rr_w_bytes : 0);
+  // stage: RR the halo (hi | lo), HALO one tap's weight tile (hi | lo), else one K block of A and W (hi | lo each);
+  // the resident weights (RR) / the two A buffers (HALO) are carved next to the barriers
+  const int stage_bytes = rr ? 2 * p.rr_a_bytes : halo ? 2 * p.BN * BK * 2 : 2 * kTileABytes + 2 * p.BN * BK * 2;
+  const int bar_bytes = kBarBytes + (rr ? p.rr_w_bytes : 0) + (halo ? 4 * p.halo_a_bytes : 0);
   int stages = (kSmemLimit - 1024 - bar_bytes) / stage_bytes;
   if (stages > kMaxStages) stages = kMaxStages;
   FFCB_REQUIRE(stages >= 2, "conv(tc): BN=%d leaves fewer than 2 pipeline stages", p.BN);
@@ -776,9 +939,13 @@ int conv_tc(const ffcb_conv_desc* d, cudaStream_t stream) {
   };
   auto launch_bn = [&](auto bn) -> int {
     constexpr int N = decltype(bn)::value;
-    if (rr) return launch(conv_tc_kernel<false, false, true, N>);
-    if (any_il) return p.out_planar ? launch(conv_tc_kernel<true, true, false, N>) : launch(conv_tc_kernel<true, false, false, N>);
-    return p.out_planar ? launch(conv_tc_kernel<false, true, false, N>) : launch(conv_tc_kernel<false, false, false, N>);
+    if (rr) return launch(conv_tc_kernel<false, false, true, false, N>);
+    if (halo) return launch(conv_tc_kernel<false, false, false, true, N>);
+    if (any_il)
+      return p.out_planar ? launch(conv_tc_kernel<true, true, false, false, N>)
+                          : launch(conv_tc_kernel<true, false, false, false, N>);
+    return p.out_planar ? launch(conv_tc_kernel<false, true, false, false, N>)
+                        : launch(conv_tc_kernel<false, false, false, false, N>);
   };
   switch (p.BN) {
     case 32: rc = launch_bn(std::integral_constant<int, 32>()); break;
