@@ -695,14 +695,11 @@ def emit_resnet_block(prog: Program, blk, X: Buf, cl: int, cg: int, in_place: bo
     return out
 
 
-# Largest plane side the forward+backward block program is used for.  Hardware-validated against autograd: 32x32 and
-# 64x64 (planar chain), 12x20 and 17x25 (general FFT kernels) — tests/test_gpu_parity.py.  A late check of round 2
-# (tools/grad_check.py) found the program's FORWARD off by 8-14 % (2-norm) on 128-wide
-# planes (128x128 and 96x128 alike, so an x-direction effect) although the CPU interpretation of the very same program
-# matches the oracle to 2e-7 and the whole-generator program is right at 128x128 and 256x256 planes: a kernel-level
-# defect specific to the standalone block program's buffers at that width, not yet located.  Until it is, planes wider
-# than 64 take the torch-autograd composition (correct, ~1.4x slower in the refinement loop).
-BLOCK_GRAD_MAX_PLANE = 64
+# Largest plane side the forward+backward block program is used for: the largest plane its input gradients are tested
+# at against autograd through the oracle (tests/test_gpu_parity.py: 32x32, 64x64, 12x20; tests/test_gpu_program_diff.py:
+# 128x128, 96x128, 256x256 and every op of the program at 128-wide planes).  Larger planes take the torch-autograd
+# composition.
+BLOCK_GRAD_MAX_PLANE = 256
 
 
 def block_grad_supported(blk) -> bool:

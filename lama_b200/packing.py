@@ -220,7 +220,7 @@ def apply_packed_reference(p: PackedConv, inputs: Sequence[torch.Tensor], out_hw
     b = inputs[0].shape[0]
     acc = torch.zeros(b, ho, wo, p.n_out, dtype=torch.float64, device=inputs[0].device)
     k0 = 0
-    w = p.w_kn.double()
+    w = p.w_kn.double().to(acc.device)          # packed on the module's device, checked wherever the data is
     ys = torch.arange(ho, device=acc.device) * p.stride
     xs = torch.arange(wo, device=acc.device) * p.stride
     for s in p.segs:
@@ -239,7 +239,7 @@ def apply_packed_reference(p: PackedConv, inputs: Sequence[torch.Tensor], out_hw
         acc += g @ w[k0:k0 + s.nch]
         k0 += s.nch
     if p.shift is not None:
-        acc += p.shift.double()
+        acc += p.shift.double().to(acc.device)
     if addend is not None and not addend_post:
         acc += addend.double()
     if p.act == L.ACT_RELU:

@@ -628,7 +628,8 @@ def test_resnet_block_input_gradients_vs_autograd_oracle(shape, math_mode):
     """SURVEY.md row f3 groundwork: dL/dx_l, dL/dx_g through a native FFCResnetBlock (torch.autograd.Function around
     the forward+backward program) vs autograd through the torch-CPU oracle port; 1e-4 (fp32 arm) / 5e-4 (split-bf16
     operands in both directions) of the gradient's range on all but the few elements behind a flipped ReLU mask.  Shapes: the verdict's (2, 128+384, 32, 32) — planar 32x32 chain —, the
-    64x64 bottleneck, and a small non-power-of-two plane on the general FFT kernels."""
+    64x64 bottleneck, and a small non-power-of-two plane on the general FFT kernels.  Wider planes (128x128, 96x128,
+    256x256, up to engine.BLOCK_GRAD_MAX_PLANE): tests/test_gpu_program_diff.py."""
     b, cl, cg, h, w = shape
     blk = seeded_parameters_(M.FFCResnetBlock(cl + cg, padding_type="reflect", norm_layer=torch.nn.BatchNorm2d,
                                               activation_layer=torch.nn.ReLU, ratio_gin=0.75, ratio_gout=0.75,
