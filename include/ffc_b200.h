@@ -38,7 +38,7 @@
 extern "C" {
 #endif
 
-#define FFCB_VERSION 111 /* 0.1.1: ffcb_tensor gained the channel-group fields cg / tile / sg */
+#define FFCB_VERSION 112 /* 0.1.2: ffcb_add, ffcb_head_bwd7 (0.1.1: ffcb_tensor gained cg / tile / sg) */
 
 enum {
   FFCB_OK = 0,
@@ -251,6 +251,26 @@ int ffcb_fill_reflect_border(const ffcb_tensor* t, ffcb_stream_t stream);
 int ffcb_relu_bwd(const ffcb_tensor* dy, const ffcb_tensor* y, const ffcb_tensor* out, ffcb_stream_t stream);
 int ffcb_fold_reflect_border(const ffcb_tensor* gpad, const ffcb_tensor* add0, int add0_c0, const ffcb_tensor* add1,
                              int add1_c0, const ffcb_tensor* out, ffcb_stream_t stream);
+
+/*
+ * Input gradients through the generator's rear (residual blocks -> ConcatTupleLayer -> up-sampling tail -> head,
+ * ffc.py:345-363; what evaluation/refinement.py:137-167 back-propagates through on every Adam step) as one program:
+ *   ffcb_add:       out = a + b elementwise over the whole padded extent (interior and ring) of three views of one
+ *                   geometry (B, H, W, C, pad); any storage format on each; `out` may alias `a`.  Replaces the block
+ *                   identity add `x_l + y_l, x_g + y_g` (ffc.py:288) where the backward needs y (= Y2, the conv2 ReLU
+ *                   output) kept apart.  Summing the reflected rings keeps out's ring a reflection of its interior.
+ *   ffcb_head_bwd7: adjoint of ReflectionPad2d(3) -> Conv2d(Cin -> N <= 4, k7) -> act (ffc.py:360-363), fused with
+ *                   the ReLU of the last up-sampling stage (ffc.py:354):
+ *                     out = [mask > 0] * Fold3(Conv7^T(act'(y) * dy))
+ *                   y, dy: the forward output and its gradient, NCHW float [B][N][H][W]; act' = y(1-y) (sigmoid),
+ *                   1-y^2 (tanh), 1 (none); w: float [N][7*7][Cin] (the layout of ffcb_head_conv7); Conv7^T scatters
+ *                   every output pixel's gradient over its 7x7 window of the (H+6)x(W+6) padded plane and Fold3 adds
+ *                   each padded position onto the interior pixel the reflection copied it from.  mask, out: (B, H, W,
+ *                   Cin) views (mask = the last up-sampling output, any ring width).  H, W >= 4.
+ */
+int ffcb_add(const ffcb_tensor* a, const ffcb_tensor* b, const ffcb_tensor* out, ffcb_stream_t stream);
+int ffcb_head_bwd7(const float* y_nchw, const float* dy_nchw, int B, int N, int H, int W, const float* w, int act,
+                   const ffcb_tensor* mask, const ffcb_tensor* out, ffcb_stream_t stream);
 
 /* number of kernel launches issued by this library on the calling thread since the last
  * ffcb_reset_launch_count() — bench.py reports it as "gpu_launches" */

@@ -82,6 +82,9 @@ int head_gather7_blend_u8(const ffcb_tensor*, const float*, int, const uint8_t*,
 int relu_bwd(const ffcb_tensor*, const ffcb_tensor*, const ffcb_tensor*, cudaStream_t);
 int fold_reflect_border(const ffcb_tensor*, const ffcb_tensor*, int, const ffcb_tensor*, int, const ffcb_tensor*,
                         cudaStream_t);
+int add(const ffcb_tensor*, const ffcb_tensor*, const ffcb_tensor*, cudaStream_t);
+int head_bwd7(const float*, const float*, int, int, int, int, const float*, int, const ffcb_tensor*, const ffcb_tensor*,
+              cudaStream_t);
 
 static int check_conv(const ffcb_conv_desc* d) {
   FFCB_REQUIRE(d != nullptr, "conv: null descriptor");
@@ -210,6 +213,15 @@ int ffcb_relu_bwd(const ffcb_tensor* dy, const ffcb_tensor* y, const ffcb_tensor
 int ffcb_fold_reflect_border(const ffcb_tensor* gpad, const ffcb_tensor* add0, int add0_c0, const ffcb_tensor* add1,
                              int add1_c0, const ffcb_tensor* out, ffcb_stream_t stream) {
   return fold_reflect_border(gpad, add0, add0_c0, add1, add1_c0, out, (cudaStream_t)stream);
+}
+
+int ffcb_add(const ffcb_tensor* a, const ffcb_tensor* b, const ffcb_tensor* out, ffcb_stream_t stream) {
+  return add(a, b, out, (cudaStream_t)stream);
+}
+
+int ffcb_head_bwd7(const float* y_nchw, const float* dy_nchw, int B, int N, int H, int W, const float* w, int act,
+                   const ffcb_tensor* mask, const ffcb_tensor* out, ffcb_stream_t stream) {
+  return head_bwd7(y_nchw, dy_nchw, B, N, H, W, w, act, mask, out, (cudaStream_t)stream);
 }
 
 long long ffcb_launch_count(void) { return g_launches; }

@@ -10,6 +10,11 @@
 //   ffcb_relu_bwd             dx = dy * [y > 0]                      (y = the forward activation, ffc.py:101,133,253-254)
 //   ffcb_fold_reflect_border  adjoint of ReflectionPad(1): the gradient w.r.t. the padded plane folded back onto the
 //                             interior (+ up to two addends: the 1x1 branch's gradient, the residual path's gradient)
+// and, for the generator's rear (residual blocks + up-sampling tail + head, lama_b200/engine.py:
+// build_rear_grad_program):
+//   ffcb_add                  out = a + b over the padded extent (the block identity X + Y2, ffc.py:288, with Y2 kept)
+//   ffcb_head_bwd7            adjoint of ReflectionPad2d(3) + Conv2d 7x7 + act (ffc.py:360-363), fused with the ReLU
+//                             mask of the last up-sampling stage (ffc.py:350-354)
 #include <stdint.h>
 
 #include "common.cuh"
@@ -82,6 +87,120 @@ int grid_for(long long total) {
   return (int)(blocks < 132 * 16 ? blocks : 132 * 16);
 }
 
+// out = a + b over the whole padded extent (interior and ring) of three views of one geometry
+__global__ void add_kernel(View a, View b, View out) {
+  const int P = out.pad, Hp = out.H + 2 * P, Wp = out.W + 2 * P, c4 = out.C / 4;
+  const long long total = (long long)out.B * Hp * Wp * c4;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int q = (int)(i % c4);
+    const long long p = i / c4;
+    const int x = (int)(p % Wp) - P, y = (int)((p / Wp) % Hp) - P, bb = (int)(p / ((long long)Wp * Hp));
+    const float4 u = load4g(a, bb, y, x, 4 * q), v = load4g(b, bb, y, x, 4 * q);
+    store4g(out, bb, y, x, 4 * q, make_float4(u.x + v.x, u.y + v.y, u.z + v.z, u.w + v.w));
+  }
+}
+
+// ---- head backward: [mask > 0] * Fold3(Conv7^T(act'(y) * dy)) --------------------------------------------------
+// One CTA: HB_TH x HB_TW interior pixels x HB_CC channels of one image.  g = act'(y) * dy of the output rows / columns
+// the tile's 7x7 windows reach ([y0-3, y0+TH+3) x [x0-3, x0+TW+3), zero outside the plane) and the tile's weights
+// stay in shared memory.  A thread owns 4 adjacent pixels x 4 channels: per (n, ky) it reads 10 g values and 7
+// weight quads for 112 FMA.
+//
+// Padded position (py, px) of the (H+6) x (W+6) plane receives  sum_{ky,kx} g[py-ky][px-kx] w[ky][kx]  and interior
+// pixel (y, x) collects every padded position ReflectionPad2d(3) copied from it: row y+3, row 3-y (1 <= y <= 3) and
+// row 2H+1-y (H-4 <= y <= H-2), the same for columns.  The main term (y+3, x+3) runs vectorised; the reflected
+// terms exist only for pixels within 4 of an edge and run per pixel.  Every g they read lies inside the tile's window
+// or outside the plane (the tiles are at least 4 rows / columns, so the first tile starts at 0 and the tile holding
+// row H-2 reaches row H-1).
+constexpr int HB_TH = 8, HB_TW = 32, HB_CC = 32, HB_GR = HB_TH + 6, HB_GC = HB_TW + 6;
+constexpr int HB_THREADS = (HB_CC / 4) * (HB_TW / 4) * HB_TH;
+
+__device__ __forceinline__ void fma4(float4& a, float g, const float4& w) {
+  a.x = __fmaf_rn(g, w.x, a.x); a.y = __fmaf_rn(g, w.y, a.y); a.z = __fmaf_rn(g, w.z, a.z); a.w = __fmaf_rn(g, w.w, a.w);
+}
+
+__global__ void __launch_bounds__(HB_THREADS) head_bwd7_kernel(const float* __restrict__ y, const float* __restrict__ dy,
+                                                               int N, int H, int W, int Cin,
+                                                               const float* __restrict__ w, int act, View mask,
+                                                               View out, int nchunk) {
+  __shared__ float g_s[4][HB_GR][HB_GC];
+  __shared__ __align__(16) float w_s[4 * 49 * HB_CC];
+  const int b = blockIdx.z / nchunk, c0 = (blockIdx.z % nchunk) * HB_CC;
+  const int cc = min(HB_CC, Cin - c0);
+  const int y0 = blockIdx.y * HB_TH, x0 = blockIdx.x * HB_TW;
+  const int tid = threadIdx.x;
+  for (int i = tid; i < N * 49 * HB_CC; i += HB_THREADS) {           // w: [N][49][Cin] -> [N][49][HB_CC]
+    const int c = i % HB_CC, nt = i / HB_CC;
+    w_s[i] = c < cc ? w[(long long)nt * Cin + c0 + c] : 0.f;
+  }
+  for (int i = tid; i < N * HB_GR * HB_GC; i += HB_THREADS) {
+    const int cx = i % HB_GC, r = (i / HB_GC) % HB_GR, n = i / (HB_GC * HB_GR);
+    const int oy = y0 - 3 + r, ox = x0 - 3 + cx;
+    float v = 0.f;
+    if (oy >= 0 && oy < H && ox >= 0 && ox < W) {
+      const long long o = (((long long)b * N + n) * H + oy) * W + ox;
+      const float yv = y[o], d = dy[o];
+      v = act == FFCB_ACT_SIGMOID ? d * (yv * (1.f - yv)) : (act == FFCB_ACT_TANH ? d * (1.f - yv * yv) : d);
+    }
+    g_s[n][r][cx] = v;
+  }
+  __syncthreads();
+  const int q = tid % (HB_CC / 4), xg = (tid / (HB_CC / 4)) % (HB_TW / 4), ty = tid / ((HB_CC / 4) * (HB_TW / 4));
+  float4 acc[4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) acc[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int n = 0; n < N; ++n) {
+#pragma unroll 1
+    for (int ky = 0; ky < 7; ++ky) {
+      float gv[10];
+#pragma unroll
+      for (int j = 0; j < 10; ++j) gv[j] = g_s[n][ty + 6 - ky][xg * 4 + j];
+      const float4* wr = reinterpret_cast<const float4*>(w_s + (n * 49 + ky * 7) * HB_CC) + q;
+#pragma unroll
+      for (int kx = 0; kx < 7; ++kx) {
+        const float4 wv = wr[kx * (HB_CC / 4)];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) fma4(acc[j], gv[j + 6 - kx], wv);
+      }
+    }
+  }
+  if (4 * q >= cc) return;
+  const int yy = y0 + ty;
+  if (yy >= H) return;
+  int rows[3], nr = 1;
+  rows[0] = yy + 3;
+  if (yy >= 1 && yy <= 3) rows[nr++] = 3 - yy;
+  if (yy >= H - 4 && yy <= H - 2) rows[nr++] = 2 * H + 1 - yy;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const int xx = x0 + xg * 4 + j;
+    if (xx >= W) break;
+    int cols[3], nc = 1;
+    cols[0] = xx + 3;
+    if (xx >= 1 && xx <= 3) cols[nc++] = 3 - xx;
+    if (xx >= W - 4 && xx <= W - 2) cols[nc++] = 2 * W + 1 - xx;
+    float4 r = acc[j];
+    for (int a = 0; a < nr; ++a)
+      for (int e = 0; e < nc; ++e) {
+        if (a == 0 && e == 0) continue;                          // the main term, done above
+        for (int n = 0; n < N; ++n)
+          for (int ky = 0; ky < 7; ++ky) {
+            const int lr = rows[a] - ky - y0 + 3;              // local row of g[py - ky]
+            if (lr < 0 || lr >= HB_GR) continue;
+            for (int kx = 0; kx < 7; ++kx) {
+              const int lc = cols[e] - kx - x0 + 3;
+              if (lc < 0 || lc >= HB_GC) continue;
+              fma4(r, g_s[n][lr][lc], reinterpret_cast<const float4*>(w_s + (n * 49 + ky * 7 + kx) * HB_CC)[q]);
+            }
+          }
+      }
+    const float4 m = load4g(mask, b, yy, xx, c0 + 4 * q);
+    store4g(out, b, yy, xx, c0 + 4 * q,
+            make_float4(m.x > 0.f ? r.x : 0.f, m.y > 0.f ? r.y : 0.f, m.z > 0.f ? r.z : 0.f, m.w > 0.f ? r.w : 0.f));
+  }
+}
+
 }  // namespace
 
 int relu_bwd(const ffcb_tensor* dy, const ffcb_tensor* y, const ffcb_tensor* out, cudaStream_t stream) {
@@ -123,6 +242,44 @@ int fold_reflect_border(const ffcb_tensor* gpad, const ffcb_tensor* add0, int ad
   if (total == 0) return FFCB_OK;
   fold_reflect_kernel<<<grid_for(total), 256, 0, stream>>>(make_view(*gpad), va, vb, make_view(*out));
   FFCB_LAUNCH_CHECK("fold_reflect_kernel");
+  return FFCB_OK;
+}
+
+int add(const ffcb_tensor* a, const ffcb_tensor* b, const ffcb_tensor* out, cudaStream_t stream) {
+  int rc;
+  if ((rc = check_tensor(a, "add.a")) || (rc = check_tensor(b, "add.b")) || (rc = check_tensor(out, "add.out")))
+    return rc;
+  for (const ffcb_tensor* t : {a, b})
+    FFCB_REQUIRE(t->B == out->B && t->H == out->H && t->W == out->W && t->C == out->C && t->pad == out->pad &&
+                     !t->window,
+                 "add: the three views must have one geometry (B, H, W, C, ring)");
+  FFCB_REQUIRE(!out->window, "add: window views are not accepted");
+  const long long total = (long long)out->B * (out->H + 2 * out->pad) * (out->W + 2 * out->pad) * (out->C / 4);
+  if (total == 0) return FFCB_OK;
+  add_kernel<<<grid_for(total), 256, 0, stream>>>(make_view(*a), make_view(*b), make_view(*out));
+  FFCB_LAUNCH_CHECK("add_kernel");
+  return FFCB_OK;
+}
+
+int head_bwd7(const float* y, const float* dy, int B, int N, int H, int W, const float* w, int act,
+              const ffcb_tensor* mask, const ffcb_tensor* out, cudaStream_t stream) {
+  int rc;
+  if ((rc = check_tensor(mask, "head_bwd7.mask")) || (rc = check_tensor(out, "head_bwd7.out"))) return rc;
+  FFCB_REQUIRE(N >= 1 && N <= 4, "head_bwd7: N=%d outside [1,4]", N);
+  FFCB_REQUIRE(act == FFCB_ACT_NONE || act == FFCB_ACT_SIGMOID || act == FFCB_ACT_TANH,
+               "head_bwd7: activation %d is not none / sigmoid / tanh", act);
+  FFCB_REQUIRE(H >= 4 && W >= 4, "head_bwd7: ReflectionPad2d(3) needs H, W >= 4 (got %dx%d)", H, W);
+  FFCB_REQUIRE(out->B == B && out->H == H && out->W == W && mask->B == B && mask->H == H && mask->W == W &&
+                   mask->C == out->C && !out->window && !mask->window,
+               "head_bwd7: out / mask must be (B, H, W, Cin) views of the output's plane");
+  FFCB_REQUIRE(y != nullptr && dy != nullptr && w != nullptr, "head_bwd7: null pointer");
+  if ((long long)B * H * W * out->C == 0) return FFCB_OK;
+  const int nchunk = (out->C + HB_CC - 1) / HB_CC;
+  FFCB_REQUIRE((long long)B * nchunk <= 65535, "head_bwd7: batch %d too large", B);
+  dim3 grid((W + HB_TW - 1) / HB_TW, (H + HB_TH - 1) / HB_TH, B * nchunk);
+  head_bwd7_kernel<<<grid, HB_THREADS, 0, stream>>>(y, dy, N, H, W, out->C, w, act, make_view(*mask),
+                                                     make_view(*out), nchunk);
+  FFCB_LAUNCH_CHECK("head_bwd7_kernel");
   return FFCB_OK;
 }
 

@@ -210,6 +210,27 @@ class FoldOp:
 
 
 @dataclass
+class AddOp:
+    """out = a + b over the whole padded extent of three views of one geometry (ffcb_add); ``out`` may be ``a``."""
+    a: TV
+    b: TV
+    out: TV
+
+
+@dataclass
+class HeadBwdOp:
+    """Adjoint of ReflectionPad2d(3) + 7x7 head + act, masked by the last up-sampling ReLU (ffcb_head_bwd7):
+    out = [mask > 0] * Fold3(Conv7^T(act'(y) * dy)), with y / dy the external NCHW output and its gradient."""
+    y: str            # external output of the forward part (the head's)
+    dy: str           # external NCHW input of the backward part
+    w: torch.Tensor   # [N][49][C] (pack_head)
+    n_out: int
+    act: int
+    mask: TV
+    out: TV
+
+
+@dataclass
 class SplitOp:
     """Boundary between the forward and the backward part of a forward+backward program (no kernel)."""
 
@@ -857,6 +878,8 @@ def build_module_program(module, kind: str, shapes: Sequence[Optional[Tuple[int,
         build_block_grad_program(prog, module, shapes[0], shapes[1])
     elif kind == "generator":
         build_generator_program(prog, module, shapes[0])
+    elif kind == "generator_rear_grad":
+        build_rear_grad_program(prog, module, shapes[0], shapes[1])
     elif kind.startswith("generator_u8"):            # "generator_u8:<pad modulo>", shapes = (img, mask)
         mod = int(kind.split(":")[1]) if ":" in kind else 8
         b, h0, w0, _ = shapes[0]
@@ -914,17 +937,9 @@ def build_generator_program(prog: Program, gen, shape, u8_size: Optional[Tuple[i
     for blk in blocks:
         X = emit_resnet_block(prog, blk, X, cl, cg, in_place=True)
     # ConcatTupleLayer (ffc.py:295-302) is free: x_l | x_g already share X.
-    tc_head = (prog.math == L.MATH_BF16X3 and head.in_channels % 8 == 0 and head.out_channels <= 3
-               and min(h, w) > 3 and os.environ.get("LAMA_B200_HEAD", "tc") == "tc")
-    for iu, (ct, bn) in enumerate(ups):
-        sc, sh = P.bn_scale_shift(bn)
-        last = iu == len(ups) - 1
-        # tensor-core head: its row contraction reads 3 pixels up and down -> ring of 3; CUDA-core head: float32
-        Yb = prog.buf("up", b, X.H * 2, X.W * 2, ct.out_channels, gemm=(not last) or tc_head,
-                      halo=(not last) or tc_head, halo_px=3 if last else 1)
-        for a, bb, pk in P.pack_conv_transpose_phases(ct.weight, ct.bias, sc, sh, act=L.ACT_RELU, device=dev):
-            prog.ops.append(ConvOp(pk, [TV(X), None], TV(Yb, phase=(a, bb)), tag=f"convT phase {a}{bb}+bn+relu"))
-        X = Yb
+    tc_head = _tc_head(prog, head, h, w)
+    ups_out = emit_up_tail(prog, ups, X, tc_head)
+    X = ups_out[-1] if ups_out else X
     if out_blk is not None:
         # out_ffc: FFCResnetBlock(inline=True) splits its input as x[:, :-g] | x[:, -g:] (ffc.py:278-280) — exactly the
         # [local | global] channel order of the buffer, so it runs in place like the bottleneck blocks
@@ -932,19 +947,131 @@ def build_generator_program(prog: Program, gen, shape, u8_size: Optional[Tuple[i
         X = emit_resnet_block(prog, out_blk, X, X.C - ocg, ocg, in_place=True)
     if u8_size is not None and not (tc_head and ups and head.out_channels == 3):
         raise ValueError("the uint8 predict path needs the tensor-core head with 3 output channels")
-    if tc_head and ups:
+    emit_head(prog, head, out_act, X, tc_head and bool(ups), u8_size)
+    prog.outputs["y0"] = (b, head.out_channels, h, w) if u8_size is None else (b, h0, w0, 3)
+
+
+def _tc_head(prog: Program, head, h: int, w: int) -> bool:
+    """The tensor-core head (row contraction + gather) applies: split-bf16 arithmetic, N <= 3, planes wider than 3."""
+    return (prog.math == L.MATH_BF16X3 and head.in_channels % 8 == 0 and head.out_channels <= 3
+            and min(h, w) > 3 and os.environ.get("LAMA_B200_HEAD", "tc") == "tc")
+
+
+def emit_up_tail(prog: Program, ups, X: Buf, tc_head: bool) -> List[Buf]:
+    """ConvTranspose2d(k3, s2, p1, op1) + BN + ReLU stages (ffc.py:350-354) as sub-pixel phases; returns the ReLU
+    output of every stage.  The last one feeds the head: with the tensor-core head its row contraction reads 3 pixels
+    up and down -> split bf16 with a ring of 3; with the CUDA-core head float32."""
+    outs = []
+    for iu, (ct, bn) in enumerate(ups):
+        sc, sh = P.bn_scale_shift(bn)
+        last = iu == len(ups) - 1
+        Yb = prog.buf("up", X.B, X.H * 2, X.W * 2, ct.out_channels, gemm=(not last) or tc_head,
+                      halo=(not last) or tc_head, halo_px=3 if last else 1)
+        for a, bb, pk in P.pack_conv_transpose_phases(ct.weight, ct.bias, sc, sh, act=L.ACT_RELU,
+                                                      device=ct.weight.device):
+            prog.ops.append(ConvOp(pk, [TV(X), None], TV(Yb, phase=(a, bb)), tag=f"convT phase {a}{bb}+bn+relu"))
+        X = Yb
+        outs.append(Yb)
+    return outs
+
+
+def emit_head(prog: Program, head, out_act: int, X: Buf, tc_head: bool, u8_size: Optional[Tuple[int, int]] = None):
+    """ReflectionPad2d(3) + Conv2d 7x7 + act (ffc.py:360-363) of ``X`` into the external output "y0"; ``u8_size``: the
+    predict path's blend / crop / uint8 variant of the tensor-core head."""
+    dev = head.weight.device
+    if tc_head:
         pkh = P.pack_head_rows(head.weight, device=dev)
-        Q = prog.buf("head.q", b, h, w, pkh.n_out)
+        Q = prog.buf("head.q", X.B, X.H, X.W, pkh.n_out)
         prog.ops.append(ConvOp(pkh, [TV(X), None], TV(Q), tag="head 7x7 rows"))
         bias = head.bias.detach().float().contiguous() if head.bias is not None else torch.zeros(head.out_channels)
         if u8_size is None:
             prog.ops.append(HeadGatherOp(TV(Q), bias.to(dev), head.out_channels, out_act, "y0"))
         else:
+            h0, w0 = u8_size
             prog.ops.append(HeadGatherU8Op(TV(Q), bias.to(dev), out_act, "img", "mask", h0, w0, "y0"))
     else:
         wh, bh = P.pack_head(head.weight, head.bias, device=dev)
         prog.ops.append(HeadOp(TV(X), wh, bh, head.out_channels, out_act, "y0"))
-    prog.outputs["y0"] = (b, head.out_channels, h, w) if u8_size is None else (b, h0, w0, 3)
+
+
+def rear_grad_supported(gen, shape_l, shape_g) -> bool:
+    """The generator's rear — residual blocks, up-sampling tail, head (``generator.model[first_block:]``) — has a
+    native forward + input-gradient program for inputs (z1, z2) of these shapes: every block has block gradients
+    (``block_grad_supported``), no out_ffc block, at least one up-sampling stage, a none / sigmoid / tanh head with
+    N <= 4, bottleneck planes up to BLOCK_GRAD_MAX_PLANE that the native FFT takes."""
+    lay = _generator_layout(gen)
+    if lay is None or shape_l is None or shape_g is None or len(shape_l) != 4 or len(shape_g) != 4:
+        return False
+    _stem, _downs, blocks, ups, out_blk, head, out_act = lay
+    if out_blk is not None or not blocks or not ups or out_act not in (L.ACT_NONE, L.ACT_SIGMOID, L.ACT_TANH):
+        return False
+    if head.out_channels > 4 or not all(block_grad_supported(b) for b in blocks):
+        return False
+    b, cl, h, w = shape_l
+    f = blocks[0].conv1.ffc
+    if (b < 1 or shape_g[0] != b or tuple(shape_g[2:]) != (h, w) or cl != f.convl2l.in_channels
+            or shape_g[1] != f.global_in_num or ups[0][0].in_channels != cl + shape_g[1]):
+        return False
+    if max(h, w) > BLOCK_GRAD_MAX_PLANE:
+        return False
+    return ffc_bn_act_shapes_ok(blocks[0].conv1, torch.empty(shape_l, device="meta"),
+                                torch.empty(shape_g, device="meta"))
+
+
+def build_rear_grad_program(prog: Program, gen, sl: Tuple[int, ...], sg: Tuple[int, ...]):
+    """``generator.model[first_block:]`` (ffc.py:345-363) forward | SplitOp | input gradients, for refinement
+    (evaluation/refinement.py:137-167 optimises z1, z2 through exactly this part).
+    inputs  x0, x1 (z1, z2: local / global halves at the bottleneck), g0 (dL/dpred, backward part);
+    outputs y0 (pred, as ``rear((z1, z2))``), dx0, dx1 (dL/dz1, dL/dz2).
+    Forward: per block conv1 -> Y1, conv2 -> its own Y2 (kept: its ReLU mask is read by the backward, which the fused
+    residual epilogue's X + Y2 would not give back), X <- X + Y2 (ffcb_add); then the generator program's tail.
+    Backward: ffcb_head_bwd7 -> for every up stage in reverse the adjoint of ConvTranspose2d(k3, s2, p1, op1): a
+    stride-2, zero-border 3x3 ffcb_conv with the transposed conv's own weight [Cin, Cout, 3, 3] (no flip) and the BN
+    scale folded along its input axis, then the ReLU mask of the stage below -> the blocks in reverse, each as two
+    FFC_BN_ACT backwards with the identity path added by the second."""
+    _stem, _downs, blocks, ups, _out_blk, head, out_act = _generator_layout(gen)
+    b, cl, h, w = sl
+    cg = sg[1]
+    dev = head.weight.device
+    prog.inputs.update(x0=tuple(sl), x1=tuple(sg))
+    X = prog.buf("in", b, h, w, cl + cg, gemm=True, halo=True)
+    prog.ops.append(ToNHWC("x0", TV(X, 0, cl)))
+    prog.ops.append(ToNHWC("x1", TV(X, cl, cg)))
+    saved = []
+    for blk in blocks:
+        Y1, _, _ = emit_ffc_bn_act(prog, blk.conv1, X, cl, cg)
+        Y2, _, _ = emit_ffc_bn_act(prog, blk.conv2, Y1, cl, cg)
+        prog.ops.append(AddOp(TV(X), TV(Y2), TV(X)))
+        saved.append((blk, Y1, Y2))
+    H, W = X.H * 2 ** len(ups), X.W * 2 ** len(ups)
+    ups_out = emit_up_tail(prog, ups, X, _tc_head(prog, head, H, W))
+    emit_head(prog, head, out_act, ups_out[-1], _tc_head(prog, head, H, W))
+    n = head.out_channels
+    prog.outputs["y0"] = (b, n, H, W)
+    prog.ops.append(SplitOp())
+    prog.inputs["g0"] = (b, n, H, W)
+    wh, _ = P.pack_head(head.weight, head.bias, device=dev)
+    D = prog.buf("grad.dup", b, H, W, head.in_channels, gemm=True)
+    prog.ops.append(HeadBwdOp("y0", "g0", wh, n, out_act, TV(ups_out[-1]), TV(D)))
+    for k in reversed(range(len(ups))):
+        ct, bn = ups[k]
+        sc, _ = P.bn_scale_shift(bn)
+        wadj = ct.weight.detach().double() * sc.double()[None, :, None, None]       # [Cin_ct, Cout_ct, 3, 3]
+        pk = P.pack_conv([(wadj, 0, 0, 1)], None, None, stride=2, border=L.BORDER_ZERO, device=dev)
+        hi, wi = ups_out[k].H // 2, ups_out[k].W // 2
+        if k > 0:
+            E_ = prog.buf("grad.up_in", b, hi, wi, ct.in_channels)
+            prog.ops.append(ConvOp(pk, [TV(D), None], TV(E_), tag=f"grad: convT{k}^T (stride 2)"))
+            D = prog.buf("grad.dup", b, hi, wi, ct.in_channels, gemm=True)
+            prog.ops.append(ReluBwdOp(TV(E_), TV(ups_out[k - 1]), TV(D)))
+        else:
+            DX = prog.buf("grad.dx", b, hi, wi, ct.in_channels)
+            prog.ops.append(ConvOp(pk, [TV(D), None], TV(DX), tag=f"grad: convT{k}^T (stride 2)"))
+    for blk, Y1, Y2 in reversed(saved):
+        D1 = emit_ffc_bn_act_backward(prog, blk.conv2, Y2, TV(DX), cl, cg)
+        DX = emit_ffc_bn_act_backward(prog, blk.conv1, Y1, TV(D1), cl, cg, extra=TV(DX))
+    prog.ops.append(ToNCHW(TV(DX, 0, cl), "dx0")); prog.outputs["dx0"] = tuple(sl)
+    prog.ops.append(ToNCHW(TV(DX, cl, cg), "dx1")); prog.outputs["dx1"] = tuple(sg)
 
 
 def tc_compatible(prog: Program) -> bool:
@@ -972,6 +1099,12 @@ def insert_border_ops(prog: Program):
         if isinstance(op, ConvOp):
             for tv in op.ins:
                 if tv is not None and tv.buf.reflect_border and id(tv.buf) in dirty:
+                    out.append(BorderOp(TV(tv.buf)))
+                    del dirty[id(tv.buf)]
+        elif isinstance(op, AddOp):
+            # ffcb_add sums the rings too: its output ring is a reflection when both input rings are
+            for tv in (op.a, op.b):
+                if tv.buf.reflect_border and id(tv.buf) in dirty:
                     out.append(BorderOp(TV(tv.buf)))
                     del dirty[id(tv.buf)]
         out.append(op)
@@ -1017,6 +1150,10 @@ def op_views(op) -> Tuple[List[TV], List[TV]]:
         return [op.dy, op.y], [op.out]
     if isinstance(op, FoldOp):
         return [op.gpad] + [tv for tv, _c0 in op.addends], [op.out]
+    if isinstance(op, AddOp):
+        return [op.a, op.b], [op.out]
+    if isinstance(op, HeadBwdOp):
+        return [op.mask], [op.out]
     if isinstance(op, SplitOp):
         return [], []
     raise TypeError(op)
@@ -1259,6 +1396,17 @@ class CudaExecutor:
             adds = [(C.byref(self._ref(self.tensor(tv))), c0) for tv, c0 in op.addends] + [(None, 0)] * 2
             self.calls.append(("ffcb_fold_reflect_border", lib.ffcb_fold_reflect_border,
                                [C.byref(g), adds[0][0], adds[0][1], adds[1][0], adds[1][1], C.byref(o)]))
+        elif isinstance(op, AddOp):
+            a, bv, o = (self._ref(self.tensor(v)) for v in (op.a, op.b, op.out))
+            self.calls.append(("ffcb_add", lib.ffcb_add, [C.byref(a), C.byref(bv), C.byref(o)]))
+        elif isinstance(op, HeadBwdOp):
+            bb, n, h, w = self.prog.inputs[op.dy]
+            m, o = self._ref(self.tensor(op.mask)), self._ref(self.tensor(op.out))
+            wd = self._dev(op.w)
+            self.input_slots.setdefault(op.dy, []).append((len(self.calls), 1))
+            self.calls.append(("ffcb_head_bwd7", lib.ffcb_head_bwd7,
+                               [self.outputs[op.y].data_ptr(), None, bb, n, h, w, wd.data_ptr(), op.act,
+                                C.byref(m), C.byref(o)]))
         elif isinstance(op, BorderOp):
             t = self._ref(self.tensor(op.view))
             self.calls.append(("ffcb_fill_reflect_border", lib.ffcb_fill_reflect_border, [C.byref(t)]))
@@ -1452,6 +1600,37 @@ class _BlockGradFn(torch.autograd.Function):
 def block_with_input_grad(module, x_l, x_g):
     """(out_l, out_g) of an FFCResnetBlock, differentiable w.r.t. x_l / x_g on the native path."""
     return _BlockGradFn.apply(module, x_l, x_g)
+
+
+class _RearGradFn(torch.autograd.Function):
+    """``generator.model[first_block:]`` — residual blocks, up-sampling tail, head — with native forward AND native
+    input gradients: the whole rear of the refinement loop (evaluation/refinement.py:137-167) as ONE
+    ``generator_rear_grad`` program per (generator, shape).  Same contract as ``_BlockGradFn``: the forward part keeps
+    its activations in the executor's buffers, and a second forward before the backward raises."""
+
+    @staticmethod
+    def forward(ctx, gen, z1, z2):
+        ex = get_executor(gen, "generator_rear_grad", (z1, z2))
+        outs = ex.run({"x0": z1.detach().contiguous(), "x1": z2.detach().contiguous()}, part=0)
+        ctx.ex, ctx.generation = ex, ex.generation
+        return outs["y0"].clone()
+
+    @staticmethod
+    def backward(ctx, gy):
+        ex = ctx.ex
+        if ex.generation != ctx.generation:
+            raise RuntimeError("lama_b200: the generator's rear ran forward again (same shape) before this backward; "
+                               "its saved activations were overwritten")
+        gy = gy.contiguous()
+        assert gy.dtype == torch.float32 and tuple(gy.shape) == tuple(ex.prog.inputs["g0"])
+        outs = ex.run({"g0": gy}, part=1)
+        return None, outs["dx0"].clone(), outs["dx1"].clone()
+
+
+def generator_rear_with_input_grad(gen, z1, z2):
+    """pred = ``gen.model[first_block:]((z1, z2))`` on the native path, differentiable w.r.t. z1 / z2 (the weights are
+    frozen).  Callers check ``rear_grad_supported(gen, z1.shape, z2.shape)`` first."""
+    return _RearGradFn.apply(gen, z1, z2)
 
 
 def run_module(module, kind: str, tensors):

@@ -1,6 +1,6 @@
 """Refinement driver for the drop-in generator (SURVEY.md row f3): the reference's multi-scale "plug-n-play" refinement
-(``saicinpainting/evaluation/refinement.py``) without kornia, on top of the native forward + input-gradient programs of
-``FFCResnetBlock`` (``lama_b200.engine.block_with_input_grad``).
+(``saicinpainting/evaluation/refinement.py``) without kornia, on top of the native forward + input-gradient program of
+the generator's rear (``lama_b200.engine.generator_rear_with_input_grad``).
 
 What the reference does (refinement.py:86-174, 228-314): build an image / mask pyramid, and at every scale optimise the
 feature maps z1, z2 entering the residual blocks (Adam, 15 iterations) so that the down-scaled prediction matches the
@@ -8,9 +8,12 @@ previous scale's result inside the (eroded) hole and the input outside.  The opt
 residual blocks, the up-sampling tail and the image-space pyramid operators; the weights are frozen.
 
 Here:
-  * residual blocks: native forward and native input gradients (eval-mode BN folded, ``torch.autograd.Function``);
+  * rear (residual blocks, ConvTranspose2d / BN / ReLU tail, 7x7 head, sigmoid): ONE native program with a forward and
+    an input-gradient part (eval-mode BN folded, ``torch.autograd.Function``), when ``engine.rear_grad_supported``
+    holds for the scale's shape; otherwise the module slice ``generator.model[first_block:]`` — native per-block
+    gradients (``engine.block_with_input_grad``) with the tail on torch autograd.  LAMA_B200_NATIVE_GRAD=0: torch
+    autograd throughout;
   * front (stem + stride-2 convs) under ``no_grad``: the native stage programs;
-  * tail (ConvTranspose2d / BN / ReLU / 7x7 head / sigmoid): torch autograd (plain ``nn`` modules of ``generator.model``);
   * pyramid operators: the three kornia calls restated with torch ops — ``gaussian_blur2d(k=5, sigma=1)`` (reflect
     border, separable normalised Gaussian), ``erosion(mask, 15x15 ellipse)`` (geodesic border: outside counts as +max,
     i.e. the border never erodes) and ``resize(bilinear, align_corners=False)``; pinned against OpenCV in
@@ -21,6 +24,7 @@ The reference pipelines the blocks over several GPUs (refinement.py:276-289); ba
 from __future__ import annotations
 
 import math
+import os
 from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -134,6 +138,31 @@ def split_generator(model: nn.Sequential):
     return model[:first], model[first:]
 
 
+class NativeRear:
+    """``rear((z1, z2))`` for ``infer_scale``: the generator's native rear program where it applies (see
+    ``engine.rear_grad_supported``), else the module slice ``generator.model[first_block:]``."""
+
+    def __init__(self, generator, modules: nn.Sequential):
+        self.generator, self.modules = generator, modules
+
+    def native_ok(self, z1, z2) -> bool:
+        from . import engine as E
+        if os.environ.get("LAMA_B200_NATIVE_GRAD", "1") == "0" or not torch.is_grad_enabled() or self.generator.training:
+            return False
+        if not all(torch.is_tensor(z) and z.is_cuda and z.dtype == torch.float32 for z in (z1, z2)):
+            return False
+        if any(p.requires_grad for p in self.generator.parameters()):
+            return False
+        return E.rear_grad_supported(self.generator, tuple(z1.shape), tuple(z2.shape))
+
+    def __call__(self, z):
+        z1, z2 = z
+        if self.native_ok(z1, z2):
+            from . import engine as E
+            return E.generator_rear_with_input_grad(self.generator, z1, z2)
+        return self.modules(z)
+
+
 def _pad_to_modulo(t: torch.Tensor, mod: int) -> torch.Tensor:
     """evaluation/data.py:36-40 (reflect padding at the bottom / right)."""
     h, w = t.shape[2:]
@@ -178,6 +207,7 @@ def refine_predict(image: torch.Tensor, mask: torch.Tensor, generator, *, modulo
     for p in generator.parameters():
         p.requires_grad_(False)                       # model.freeze(): input gradients only
     front, rear = split_generator(generator.model)
+    rear = NativeRear(generator, rear)
     images, masks = image_mask_pyramid(image, mask, min_side, max_scales, px_budget)
     result = None
     for im, mk in zip(images, masks):
