@@ -38,7 +38,7 @@
 extern "C" {
 #endif
 
-#define FFCB_VERSION 112 /* 0.1.2: ffcb_add, ffcb_head_bwd7 (0.1.1: ffcb_tensor gained cg / tile / sg) */
+#define FFCB_VERSION 113 /* 0.1.3: ffcb_refine_l1_grad (0.1.2: ffcb_add, ffcb_head_bwd7; 0.1.1: ffcb_tensor gained cg / tile / sg) */
 
 enum {
   FFCB_OK = 0,
@@ -271,6 +271,27 @@ int ffcb_fold_reflect_border(const ffcb_tensor* gpad, const ffcb_tensor* add0, i
 int ffcb_add(const ffcb_tensor* a, const ffcb_tensor* b, const ffcb_tensor* out, ffcb_stream_t stream);
 int ffcb_head_bwd7(const float* y_nchw, const float* dy_nchw, int B, int N, int H, int W, const float* w, int act,
                    const ffcb_tensor* mask, const ffcb_tensor* out, ffcb_stream_t stream);
+
+/*
+ * Gradient of the refinement loss w.r.t. the prediction (evaluation/refinement.py:75-84 _l1_loss, 19-26 _pyrdown,
+ * 151-158 the loss of one Adam step), per image b of NCHW float32 tensors:
+ *   L_b = mean_{c,p: mask < 1e-8} |pred - image|                      over the padded plane (B, C, Hp, Wp)
+ *       + mean_{c,q: md >= 1e-8} |D(pred[:, :, :H0, :W0]) - ref|       ref (B, C, H0/2, W0/2), md (B, 1, H0/2, W0/2)
+ *   D   = bilinear (align_corners=False, source max(scale (d + 0.5) - 0.5, 0), scale = in / out) to (H0/2, W0/2)
+ *         with the source index and weights computed as torch's double-precision interpolate does (then rounded
+ *         to float); torch's float32 interpolate computes them in float, which differs by up to ~1e-5 at d ~ 100
+ *         o 5x5 separable Gaussian with reflect-101 padding (kornia's gaussian_blur2d, border 'reflect')
+ *   grad = dL_b / dpred = sign(pred - image) [mask < 1e-8] inv_n[b][0]
+ *                         + D^T(sign(D pred - ref) [md >= 1e-8] inv_n[b][1])        (zero outside the crop)
+ * mask (B, 1, Hp, Wp); inv_n (B, 2) device floats 1 / n_out, 1 / n_down with n = C x the selected pixel count, 0 for
+ * an empty selection (that term then adds no gradient and its loss is NaN, as torch.mean of nothing); taps: the 5
+ * float Gaussian taps; work: B*C*(H0/2)*(W0/2) floats of scratch.  loss (B, 2): the two terms (reported only, summed
+ * with atomics).  sign(0) = 0.  The gradient is a fixed-order gather per element: no atomics, batch-independent.
+ * C in [1, 4], 3 <= H0 <= Hp, 3 <= W0 <= Wp.
+ */
+int ffcb_refine_l1_grad(const float* pred, const float* image, const float* mask, int B, int C, int Hp, int Wp, int H0,
+                        int W0, const float* ref, const float* md, const float* inv_n, const float* taps, float* work,
+                        float* grad, float* loss, ffcb_stream_t stream);
 
 /* number of kernel launches issued by this library on the calling thread since the last
  * ffcb_reset_launch_count() — bench.py reports it as "gpu_launches" */

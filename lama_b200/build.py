@@ -16,7 +16,8 @@ LIB_PATH = os.path.join(HERE, "libffc_b200.so")
 STAMP = LIB_PATH + ".stamp"
 OBJ_DIR = os.path.join(HERE, "build")
 
-SOURCES = ["api.cu", "fft.cu", "fft_plane.cu", "fft_plane_cg.cu", "conv_simt.cu", "conv_tc.cu", "shell.cu", "grad.cu"]
+SOURCES = ["api.cu", "fft.cu", "fft_plane.cu", "fft_plane_cg.cu", "conv_simt.cu", "conv_tc.cu", "shell.cu", "grad.cu",
+           "refine.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + [
     "-O3", "-std=c++17", "-lineinfo", "--expt-relaxed-constexpr",

@@ -85,6 +85,8 @@ int fold_reflect_border(const ffcb_tensor*, const ffcb_tensor*, int, const ffcb_
 int add(const ffcb_tensor*, const ffcb_tensor*, const ffcb_tensor*, cudaStream_t);
 int head_bwd7(const float*, const float*, int, int, int, int, const float*, int, const ffcb_tensor*, const ffcb_tensor*,
               cudaStream_t);
+int refine_l1_grad(const float*, const float*, const float*, int, int, int, int, int, int, const float*, const float*,
+                   const float*, const float*, float*, float*, float*, cudaStream_t);
 
 static int check_conv(const ffcb_conv_desc* d) {
   FFCB_REQUIRE(d != nullptr, "conv: null descriptor");
@@ -222,6 +224,13 @@ int ffcb_add(const ffcb_tensor* a, const ffcb_tensor* b, const ffcb_tensor* out,
 int ffcb_head_bwd7(const float* y_nchw, const float* dy_nchw, int B, int N, int H, int W, const float* w, int act,
                    const ffcb_tensor* mask, const ffcb_tensor* out, ffcb_stream_t stream) {
   return head_bwd7(y_nchw, dy_nchw, B, N, H, W, w, act, mask, out, (cudaStream_t)stream);
+}
+
+int ffcb_refine_l1_grad(const float* pred, const float* image, const float* mask, int B, int C, int Hp, int Wp, int H0,
+                        int W0, const float* ref, const float* md, const float* inv_n, const float* taps, float* work,
+                        float* grad, float* loss, ffcb_stream_t stream) {
+  return refine_l1_grad(pred, image, mask, B, C, Hp, Wp, H0, W0, ref, md, inv_n, taps, work, grad, loss,
+                        (cudaStream_t)stream);
 }
 
 long long ffcb_launch_count(void) { return g_launches; }

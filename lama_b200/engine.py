@@ -17,6 +17,7 @@ product path below only ever executes through the CUDA library.
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence, Tuple
@@ -228,6 +229,25 @@ class HeadBwdOp:
     act: int
     mask: TV
     out: TV
+
+
+@dataclass
+class RefineLossOp:
+    """Gradient of the refinement loss w.r.t. the prediction, and its two terms (ffcb_refine_l1_grad): every operand
+    is an external NCHW tensor of the program — ``pred`` and the outputs ``grad`` / ``loss`` are program outputs, the
+    rest per-scale inputs (image, mask, ref, md, inv = 1 / n per image and term)."""
+    pred: str
+    image: str
+    mask: str
+    ref: str
+    md: str
+    inv: str
+    h0: int
+    w0: int
+    taps: torch.Tensor    # the 5 float32 Gaussian taps (refine.gaussian_kernel1d)
+    grad: str
+    loss: str
+    ref_numel: int        # B * C * (H0/2) * (W0/2): the kernel's low-resolution scratch
 
 
 @dataclass
@@ -880,6 +900,11 @@ def build_module_program(module, kind: str, shapes: Sequence[Optional[Tuple[int,
         build_generator_program(prog, module, shapes[0])
     elif kind == "generator_rear_grad":
         build_rear_grad_program(prog, module, shapes[0], shapes[1])
+    elif kind == "generator_rear":                       # the rear's forward alone (lowest refinement scale)
+        emit_rear_forward(prog, module, shapes[0], shapes[1])
+    elif kind.startswith("generator_refine:"):          # "generator_refine:<H0>x<W0>" (crop of the prediction)
+        h0, w0 = (int(v) for v in kind.split(":")[1].split("x"))
+        build_refine_program(prog, module, shapes[0], shapes[1], (h0, w0))
     elif kind.startswith("generator_u8"):            # "generator_u8:<pad modulo>", shapes = (img, mask)
         mod = int(kind.split(":")[1]) if ":" in kind else 8
         b, h0, w0, _ = shapes[0]
@@ -1023,16 +1048,20 @@ def build_rear_grad_program(prog: Program, gen, sl: Tuple[int, ...], sg: Tuple[i
     (evaluation/refinement.py:137-167 optimises z1, z2 through exactly this part).
     inputs  x0, x1 (z1, z2: local / global halves at the bottleneck), g0 (dL/dpred, backward part);
     outputs y0 (pred, as ``rear((z1, z2))``), dx0, dx1 (dL/dz1, dL/dz2).
-    Forward: per block conv1 -> Y1, conv2 -> its own Y2 (kept: its ReLU mask is read by the backward, which the fused
-    residual epilogue's X + Y2 would not give back), X <- X + Y2 (ffcb_add); then the generator program's tail.
-    Backward: ffcb_head_bwd7 -> for every up stage in reverse the adjoint of ConvTranspose2d(k3, s2, p1, op1): a
-    stride-2, zero-border 3x3 ffcb_conv with the transposed conv's own weight [Cin, Cout, 3, 3] (no flip) and the BN
-    scale folded along its input axis, then the ReLU mask of the stage below -> the blocks in reverse, each as two
-    FFC_BN_ACT backwards with the identity path added by the second."""
+    Forward: ``emit_rear_forward``; backward: ``emit_rear_backward``."""
+    fwd = emit_rear_forward(prog, gen, sl, sg)
+    prog.ops.append(SplitOp())
+    prog.inputs["g0"] = prog.outputs["y0"]
+    emit_rear_backward(prog, gen, fwd, "g0")
+
+
+def emit_rear_forward(prog: Program, gen, sl: Tuple[int, ...], sg: Tuple[int, ...]) -> dict:
+    """Forward part of the rear programs: inputs x0, x1 (z1, z2) -> output y0 (pred).  Per block conv1 -> Y1, conv2 ->
+    its own Y2 (kept: its ReLU mask is read by the backward, which the fused residual epilogue's X + Y2 would not give
+    back), X <- X + Y2 (ffcb_add); then the generator program's tail.  Returns what the backward reads."""
     _stem, _downs, blocks, ups, _out_blk, head, out_act = _generator_layout(gen)
     b, cl, h, w = sl
     cg = sg[1]
-    dev = head.weight.device
     prog.inputs.update(x0=tuple(sl), x1=tuple(sg))
     X = prog.buf("in", b, h, w, cl + cg, gemm=True, halo=True)
     prog.ops.append(ToNHWC("x0", TV(X, 0, cl)))
@@ -1046,13 +1075,25 @@ def build_rear_grad_program(prog: Program, gen, sl: Tuple[int, ...], sg: Tuple[i
     H, W = X.H * 2 ** len(ups), X.W * 2 ** len(ups)
     ups_out = emit_up_tail(prog, ups, X, _tc_head(prog, head, H, W))
     emit_head(prog, head, out_act, ups_out[-1], _tc_head(prog, head, H, W))
+    prog.outputs["y0"] = (b, head.out_channels, H, W)
+    return dict(sl=tuple(sl), sg=tuple(sg), saved=saved, ups_out=ups_out)
+
+
+def emit_rear_backward(prog: Program, gen, fwd: dict, dy: str):
+    """Input-gradient part of the rear programs, from ``dy`` (the NCHW gradient w.r.t. y0: an external input or an
+    output another op of the program writes) to the outputs dx0, dx1: ffcb_head_bwd7 -> for every up stage in reverse
+    the adjoint of ConvTranspose2d(k3, s2, p1, op1): a stride-2, zero-border 3x3 ffcb_conv with the transposed conv's
+    own weight [Cin, Cout, 3, 3] (no flip) and the BN scale folded along its input axis, then the ReLU mask of the stage
+    below -> the blocks in reverse, each as two FFC_BN_ACT backwards with the identity path added by the second."""
+    _stem, _downs, _blocks, ups, _out_blk, head, out_act = _generator_layout(gen)
+    sl, sg, saved, ups_out = fwd["sl"], fwd["sg"], fwd["saved"], fwd["ups_out"]
+    b, cl, cg = sl[0], sl[1], sg[1]
+    H, W = ups_out[-1].H, ups_out[-1].W
+    dev = head.weight.device
     n = head.out_channels
-    prog.outputs["y0"] = (b, n, H, W)
-    prog.ops.append(SplitOp())
-    prog.inputs["g0"] = (b, n, H, W)
     wh, _ = P.pack_head(head.weight, head.bias, device=dev)
     D = prog.buf("grad.dup", b, H, W, head.in_channels, gemm=True)
-    prog.ops.append(HeadBwdOp("y0", "g0", wh, n, out_act, TV(ups_out[-1]), TV(D)))
+    prog.ops.append(HeadBwdOp("y0", dy, wh, n, out_act, TV(ups_out[-1]), TV(D)))
     for k in reversed(range(len(ups))):
         ct, bn = ups[k]
         sc, _ = P.bn_scale_shift(bn)
@@ -1072,6 +1113,37 @@ def build_rear_grad_program(prog: Program, gen, sl: Tuple[int, ...], sg: Tuple[i
         DX = emit_ffc_bn_act_backward(prog, blk.conv1, Y1, TV(D1), cl, cg, extra=TV(DX))
     prog.ops.append(ToNCHW(TV(DX, 0, cl), "dx0")); prog.outputs["dx0"] = tuple(sl)
     prog.ops.append(ToNCHW(TV(DX, cl, cg), "dx1")); prog.outputs["dx1"] = tuple(sg)
+
+
+def refine_supported(gen, shape_l, shape_g, crop: Tuple[int, int]) -> bool:
+    """The refinement step program (``build_refine_program``) exists: the rear program does
+    (``rear_grad_supported``), the head writes 3 channels (the image's), and the crop (H0, W0) lies inside the
+    prediction and is at least 3x3 (the Gaussian's reflect padding of 2)."""
+    if not rear_grad_supported(gen, shape_l, shape_g):
+        return False
+    lay = _generator_layout(gen)
+    H, W = shape_l[2] * 2 ** len(lay[3]), shape_l[3] * 2 ** len(lay[3])
+    return lay[5].out_channels == 3 and 3 <= crop[0] <= H and 3 <= crop[1] <= W
+
+
+def build_refine_program(prog: Program, gen, sl: Tuple[int, ...], sg: Tuple[int, ...], crop: Tuple[int, int]):
+    """One Adam step of the refinement loop (evaluation/refinement.py:137-167) without the optimiser:
+    rear forward | SplitOp | RefineLossOp | rear backward.
+    inputs  x0, x1 (z1, z2), and the per-scale constants image (B,3,H,W), mask (B,1,H,W) in {0,1}, ref (B,3,H0/2,W0/2),
+            md (B,1,H0/2,W0/2) (the eroded down-scaled mask), inv (B,2) (1 / n_out, 1 / n_down, 0 for an empty term);
+    outputs y0 (pred), dy0 (dL/dpred, written by RefineLossOp and read by the head adjoint), loss (B,2), dx0, dx1.
+    ``run(part=0)`` alone is the forward-only rear (the last forward of a scale, and the lowest scale)."""
+    from .refine import gaussian_kernel1d
+    h0, w0 = crop
+    fwd = emit_rear_forward(prog, gen, sl, sg)
+    b, n, H, W = prog.outputs["y0"]
+    prog.ops.append(SplitOp())
+    prog.inputs.update(image=(b, n, H, W), mask=(b, 1, H, W), ref=(b, n, h0 // 2, w0 // 2),
+                       md=(b, 1, h0 // 2, w0 // 2), inv=(b, 2))
+    prog.outputs.update(dy0=(b, n, H, W), loss=(b, 2))
+    prog.ops.append(RefineLossOp("y0", "image", "mask", "ref", "md", "inv", h0, w0, gaussian_kernel1d(5, 1.0),
+                                 "dy0", "loss", b * n * (h0 // 2) * (w0 // 2)))
+    emit_rear_backward(prog, gen, fwd, "dy0")
 
 
 def tc_compatible(prog: Program) -> bool:
@@ -1154,7 +1226,7 @@ def op_views(op) -> Tuple[List[TV], List[TV]]:
         return [op.a, op.b], [op.out]
     if isinstance(op, HeadBwdOp):
         return [op.mask], [op.out]
-    if isinstance(op, SplitOp):
+    if isinstance(op, (SplitOp, RefineLossOp)):         # RefineLossOp reads and writes external tensors only
         return [], []
     raise TypeError(op)
 
@@ -1162,6 +1234,37 @@ def op_views(op) -> Tuple[List[TV], List[TV]]:
 def storage_key(b: Buf) -> tuple:
     """Buffers with equal keys have byte-identical storage (dtype, shape, ring, layout)."""
     return (b.fmt, b.B, b.H, b.W, b.C, b.pad, b.reflect_border, b.cg, b.tile)
+
+
+def storage_shape(b: Buf) -> Tuple[int, ...]:
+    """Shape of a buffer's storage tensor: float32, or bfloat16 with a leading 2 (hi / lo halves) for split bf16."""
+    if b.tile:
+        return (-(-(b.B * b.H * b.W) // 128), b.C // 8, 128, 8)      # zero-initialised: the tail block stays finite
+    if b.cg:
+        return (b.C // b.cg, b.B, b.H, b.W, b.cg)
+    return (b.B, b.H + 2 * b.pad, b.W + 2 * b.pad, b.C)
+
+
+def op_scratch_bytes(op) -> int:
+    """Device scratch an op's binding allocates besides the program's buffers."""
+    if isinstance(op, RefineLossOp):
+        return 4 * op.ref_numel
+    return 0
+
+
+def program_storage_bytes(prog: Program) -> int:
+    """Device bytes a ``CudaExecutor`` of ``prog`` allocates for activations, computed from the buffer shapes and
+    storage slots before anything is allocated: the pooled buffers, the FFT workspace, the program's outputs and op
+    scratch (packed weights, a few MB, are not counted).  Used to size refinement batches."""
+    slots = assign_storage_slots(prog)
+    seen, total = set(), 0
+    for b in prog.bufs:
+        if slots[b.name] not in seen:
+            seen.add(slots[b.name])
+            total += 4 * math.prod(storage_shape(b))           # float32, or two bfloat16 halves
+    for name, shape in prog.outputs.items():
+        total += math.prod(shape) * (1 if prog.dtypes.get(name, torch.float32) == torch.uint8 else 4)
+    return total + max(prog.fft_workspace_bytes(), 16) + sum(op_scratch_bytes(op) for op in prog.ops)
 
 
 def assign_storage_slots(prog: Program) -> Dict[str, int]:
@@ -1216,11 +1319,7 @@ class CudaExecutor:
             if si in slot_tensor:
                 self.storage[b.name] = slot_tensor[si]
                 continue
-            shape = (b.B, b.H + 2 * b.pad, b.W + 2 * b.pad, b.C)
-            if b.cg:
-                shape = (b.C // b.cg, b.B, b.H, b.W, b.cg)
-            if b.tile:
-                shape = (-(-(b.B * b.H * b.W) // 128), b.C // 8, 128, 8)      # zero-initialised: the tail block stays finite
+            shape = storage_shape(b)
             if b.fmt == L.F32:
                 slot_tensor[si] = torch.empty(shape, dtype=torch.float32, device=device)
             else:
@@ -1400,13 +1499,28 @@ class CudaExecutor:
             a, bv, o = (self._ref(self.tensor(v)) for v in (op.a, op.b, op.out))
             self.calls.append(("ffcb_add", lib.ffcb_add, [C.byref(a), C.byref(bv), C.byref(o)]))
         elif isinstance(op, HeadBwdOp):
-            bb, n, h, w = self.prog.inputs[op.dy]
+            bb, n, h, w = self.prog.outputs[op.y]
             m, o = self._ref(self.tensor(op.mask)), self._ref(self.tensor(op.out))
             wd = self._dev(op.w)
-            self.input_slots.setdefault(op.dy, []).append((len(self.calls), 1))
+            dy = None
+            if op.dy in self.outputs:          # written by an earlier op of the program (RefineLossOp)
+                dy = self.outputs[op.dy].data_ptr()
+            else:
+                self.input_slots.setdefault(op.dy, []).append((len(self.calls), 1))
             self.calls.append(("ffcb_head_bwd7", lib.ffcb_head_bwd7,
-                               [self.outputs[op.y].data_ptr(), None, bb, n, h, w, wd.data_ptr(), op.act,
+                               [self.outputs[op.y].data_ptr(), dy, bb, n, h, w, wd.data_ptr(), op.act,
                                 C.byref(m), C.byref(o)]))
+        elif isinstance(op, RefineLossOp):
+            bb, n, hp, wp = self.prog.outputs[op.pred]
+            work = self._dev(torch.empty(op.ref_numel, dtype=torch.float32))
+            taps = self._dev(op.taps.float())
+            i = len(self.calls)
+            for name, ai in ((op.image, 1), (op.mask, 2), (op.ref, 9), (op.md, 10), (op.inv, 11)):
+                self.input_slots.setdefault(name, []).append((i, ai))
+            self.calls.append(("ffcb_refine_l1_grad", lib.ffcb_refine_l1_grad,
+                               [self.outputs[op.pred].data_ptr(), None, None, bb, n, hp, wp, op.h0, op.w0, None, None,
+                                None, taps.data_ptr(), work.data_ptr(), self.outputs[op.grad].data_ptr(),
+                                self.outputs[op.loss].data_ptr()]))
         elif isinstance(op, BorderOp):
             t = self._ref(self.tensor(op.view))
             self.calls.append(("ffcb_fill_reflect_border", lib.ffcb_fill_reflect_border, [C.byref(t)]))

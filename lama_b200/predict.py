@@ -171,9 +171,10 @@ def shard_pairs(pairs: Sequence, rank: int, world: int) -> List:
     return list(pairs[rank::world])
 
 
-def predict_directory(inpainter: BatchedInpainter, indir: str, outdir: str, img_suffix: str = ".png",
+def predict_directory(inpainter, indir: str, outdir: str, img_suffix: str = ".png",
                       out_ext: str = ".png", chunk: int = 256, rank: int = 0, world: int = 1) -> int:
-    """bin/predict.py:63-95 for a whole directory: same file discovery and output naming, batched execution."""
+    """bin/predict.py:63-95 for a whole directory: same file discovery and output naming, batched execution.
+    ``inpainter``: a BatchedInpainter or a lama_b200.refine.BatchedRefiner (anything with ``inpaint(items)``)."""
     from PIL import Image
     if not indir.endswith("/"):
         indir += "/"
@@ -188,24 +189,52 @@ def predict_directory(inpainter: BatchedInpainter, indir: str, outdir: str, img_
     return len(pairs)
 
 
-def main(argv=None):
-    ap = argparse.ArgumentParser(description="batched LaMa inpainting on the native H100 path")
+def build_parser() -> argparse.ArgumentParser:
+    ap = argparse.ArgumentParser(
+        description="batched LaMa inpainting on the native H100 path",
+        epilog="Several GPUs: one process per GPU (python -m torch.distributed.run --nproc-per-node N -m "
+               "lama_b200.predict ...), each taking its share of the files.  With --refine this replaces the "
+               "reference's refiner.gpu_ids, which splits one image's residual blocks over several GPUs.")
     ap.add_argument("--model-dir", required=True, help="directory with config.yaml and models/<checkpoint>")
     ap.add_argument("--checkpoint", default="best.ckpt")
     ap.add_argument("--indir", required=True)
     ap.add_argument("--outdir", required=True)
     ap.add_argument("--img-suffix", default=".png")
     ap.add_argument("--out-ext", default=".png")
-    ap.add_argument("--batch", type=int, default=32)
-    ap.add_argument("--pad-mod", type=int, default=8)
-    a = ap.parse_args(argv)
+    ap.add_argument("--batch", type=int, default=32,
+                    help="images per batch (with --refine: the most; smaller when the step program would not fit)")
+    ap.add_argument("--pad-mod", type=int, default=8, help="pad to a multiple of this (the refiner's modulo too)")
+    # configs/prediction/default.yaml: refine, refiner.{n_iters, lr, min_side, max_scales, px_budget}
+    ap.add_argument("--refine", action="store_true",
+                    help="multi-scale refinement (evaluation/refinement.py) of every image: lama_b200.refine."
+                         "BatchedRefiner; images above --px-budget pixels come out at the reduced size")
+    ap.add_argument("--n-iters", type=int, default=15, help="refinement: Adam iterations per scale")
+    ap.add_argument("--lr", type=float, default=0.002, help="refinement: Adam learning rate")
+    ap.add_argument("--min-side", type=int, default=512, help="refinement: smallest side of the lowest scale")
+    ap.add_argument("--max-scales", type=int, default=3, help="refinement: most pyramid scales")
+    ap.add_argument("--px-budget", type=int, default=1800000, help="refinement: larger images are resized to this")
+    return ap
+
+
+def refiner_kwargs(a: argparse.Namespace) -> Dict:
+    """Command-line arguments -> lama_b200.refine.BatchedRefiner keyword arguments."""
+    return dict(max_batch=a.batch, modulo=a.pad_mod, n_iters=a.n_iters, lr=a.lr, min_side=a.min_side,
+                max_scales=a.max_scales, px_budget=a.px_budget)
+
+
+def main(argv=None):
+    a = build_parser().parse_args(argv)
     # one process per GPU (python -m torch.distributed.run --nproc-per-node N -m lama_b200.predict ...): every rank
     # takes its share of the files; single-process runs see rank 0 of 1
     rank, world = int(os.environ.get("RANK", "0")), int(os.environ.get("WORLD_SIZE", "1"))
     device = f"cuda:{os.environ.get('LOCAL_RANK', '0')}"
     gen = load_generator(a.model_dir, a.checkpoint, device=device)
-    n = predict_directory(BatchedInpainter(gen, max_batch=a.batch, pad_mod=a.pad_mod), a.indir, a.outdir,
-                          a.img_suffix, a.out_ext, rank=rank, world=world)
+    if a.refine:
+        from .refine import BatchedRefiner
+        inpainter = BatchedRefiner(gen, **refiner_kwargs(a))
+    else:
+        inpainter = BatchedInpainter(gen, max_batch=a.batch, pad_mod=a.pad_mod)
+    n = predict_directory(inpainter, a.indir, a.outdir, a.img_suffix, a.out_ext, rank=rank, world=world)
     print(f"[rank {rank}/{world}] inpainted {n} images -> {a.outdir}")
 
 

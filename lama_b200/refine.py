@@ -217,3 +217,260 @@ def refine_predict(image: torch.Tensor, mask: torch.Tensor, generator, *, modulo
         result = infer_scale(im_p, mk_p, front, rear, result, orig, n_iters, lr)
         result = result[:, :, :orig[0], :orig[1]]
     return result.cpu()
+
+
+# ------------------------------------------------------------------------------------------- batched refinement
+class _StepLane:
+    """One refinement step program (``engine.build_refine_program``) for a batch shape and crop, its static inputs,
+    Adam over the static z1 / z2 with ``z.grad`` bound to the program's dx outputs, and the CUDA graph of one step
+    (rear forward, loss gradient, rear backward, Adam), captured on first use and replayed for every later batch and
+    scale of the same shape."""
+
+    def __init__(self, gen, sl, sg, crop, lr: float, device, graphs: bool = True):
+        from . import engine as E
+        with torch.no_grad():
+            prog = E.build_module_program(gen, f"generator_refine:{crop[0]}x{crop[1]}", (sl, sg), E.default_math())
+        self.ex = E.CudaExecutor(prog, device)
+        self.inputs = {k: torch.zeros(v, dtype=torch.float32, device=device) for k, v in prog.inputs.items()}
+        self.z = [self.inputs["x0"].requires_grad_(True), self.inputs["x1"].requires_grad_(True)]
+        self.z[0].grad, self.z[1].grad = self.ex.outputs["dx0"], self.ex.outputs["dx1"]
+        self.opt = torch.optim.Adam(self.z, lr=lr, capturable=True)
+        self.graphs, self.graph = graphs, None
+
+    def _step(self):
+        self.ex.run(self.inputs, part=0)
+        self.ex.run(self.inputs, part=1)
+        self.opt.step()
+
+    def run(self, z1, z2, consts, n_steps: int) -> torch.Tensor:
+        """Load z1, z2 and the scale's constants, take ``n_steps`` Adam steps from a fresh optimiser state, and return
+        the forward of the final z (the executor's own y0 tensor)."""
+        with torch.no_grad():
+            self.z[0].copy_(z1)
+            self.z[1].copy_(z2)
+            for k, v in consts.items():
+                self.inputs[k].copy_(v)
+            for st in self.opt.state.values():          # every batch starts from step 0 with zero moments
+                for t in st.values():
+                    t.zero_()
+        if n_steps > 0 and (self.graph is None or not self.graphs):
+            self._step()                                # eager (the first one also creates the Adam state)
+            n_steps -= 1
+            if self.graphs:
+                self.graph = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(self.graph):
+                    self._step()
+        for _ in range(n_steps):
+            if self.graphs:
+                self.graph.replay()
+            else:
+                self._step()
+        return self.ex.run(self.inputs, part=0)["y0"]
+
+
+class _ForwardLane:
+    """The forward-only rear program (``engine.emit_rear_forward``, kind ``generator_rear``) for the lowest scale, where
+    the reference takes one forward and no step (refinement.py:150-151: no reference image yet)."""
+
+    graph = None
+
+    def __init__(self, gen, sl, sg, device):
+        from . import engine as E
+        with torch.no_grad():
+            prog = E.build_module_program(gen, "generator_rear", (sl, sg), E.default_math())
+        self.ex = E.CudaExecutor(prog, device)
+
+    def run(self, z1, z2, consts, n_steps: int) -> torch.Tensor:
+        assert n_steps == 0
+        return self.ex.run({"x0": z1.contiguous(), "x1": z2.contiguous()})["y0"]
+
+
+class BatchedRefiner:
+    """refine_predict (evaluation/refinement.py:228-314) for many images: equally sized images are refined together,
+    each scale of a batch is one step program whose forward + loss gradient + backward + Adam step is one CUDA graph
+    replayed ``n_iters - 1`` times, with no host synchronisation inside a scale.  Images do not interact (eval-mode BN,
+    per-plane FFTs, per-image losses, elementwise Adam): each gets the result it would get alone.
+
+        ref = BatchedRefiner(generator.cuda().eval(), max_batch=8)
+        outs = ref.inpaint([(img0, mask0), ...])          # HxWx3 / HxW uint8 in, HxWx3 uint8 out
+
+    Images above ``px_budget`` pixels are refined, and returned, at the reduced size, as by the reference.  Groups whose
+    scales the native step program does not cover (``engine.refine_supported``: LFU, out_ffc or gated generators,
+    bottleneck planes above ``engine.BLOCK_GRAD_MAX_PLANE``), and every group under LAMA_B200_NATIVE_GRAD=0, run
+    ``refine_predict`` image by image.  ``mem_budget``: device bytes the programs of one batch, every scale's, may pool
+    (default: 70 % of the free device memory when the group starts).  A group is cut into balanced batches, and the
+    programs of one batch size are released before those of another are built, so no more than one batch's programs are
+    alive at a time."""
+
+    def __init__(self, generator, max_batch: int = 8, *, modulo: int = 8, n_iters: int = 15, lr: float = 0.002,
+                 min_side: int = 512, max_scales: int = 3, px_budget: int = 1800000,
+                 mem_budget: Optional[int] = None):
+        self.generator = generator.eval()
+        self.device = next(generator.parameters()).device
+        if self.device.type != "cuda":
+            raise RuntimeError("BatchedRefiner needs the generator on a CUDA device (there is no CPU path)")
+        for p in generator.parameters():
+            p.requires_grad_(False)                     # model.freeze(): input gradients only
+        self.max_batch = int(max_batch)
+        self.kw = dict(modulo=modulo, n_iters=n_iters, lr=lr, min_side=min_side, max_scales=max_scales,
+                       px_budget=px_budget)
+        self.mem_budget = mem_budget
+        self.front, _ = split_generator(generator.model)
+        self._lanes = {}
+        self._size = None                               # input size the lanes in _lanes serve
+        self._graphs = True
+
+    # -- planning (pure host logic, unit-tested on CPU)
+    @staticmethod
+    def plan_batches(idx: Sequence[int], per_image_bytes: int, budget: int, max_batch: int) -> List[List[int]]:
+        """Balanced batches of ``idx`` (sizes differ by at most one) whose programs (``per_image_bytes`` per image, all
+        scales) fit ``budget``; at least one image per batch.  A program of B images pools at most B times the
+        one-image program: every buffer, output and workspace scales with B, and tile-blocked buffers round B*H*W up to
+        128 pixels once rather than per image."""
+        n = len(idx)
+        if n == 0:
+            return []
+        nb = max(1, min(int(max_batch), int(budget) // max(1, int(per_image_bytes))))
+        k = -(-n // nb)
+        sizes = [n // k + (1 if j < n % k else 0) for j in range(k)]
+        starts = [sum(sizes[:j]) for j in range(k)]
+        return [list(idx[a:a + m]) for a, m in zip(starts, sizes)]
+
+    def scale_shapes(self, h: int, w: int) -> List[Tuple[Tuple[int, ...], Tuple[int, ...], Tuple[int, int]]]:
+        """(z1 shape, z2 shape, crop) of one image per scale of an (h, w) input, lowest resolution first."""
+        from . import engine as E
+        px = self.kw["px_budget"]
+        if h * w > px:
+            ratio = math.sqrt(px / float(h * w))
+            h, w = int(h * ratio), int(w * ratio)
+        n_scales = min(1 + int(round(max(0, math.log2(min(h, w) / self.kw["min_side"])))), self.kw["max_scales"])
+        crops = [(h, w)]
+        for _ in range(n_scales - 1):
+            crops.append((crops[-1][0] // 2, crops[-1][1] // 2))
+        lay = E._generator_layout(self.generator)
+        if lay is None:
+            return []
+        blk = lay[2][0].conv1.ffc if lay[2] else None
+        f = 2 ** len(lay[1])
+        out = []
+        for h0, w0 in crops[::-1]:
+            m = self.kw["modulo"]
+            hp, wp = h0 + (-h0) % m, w0 + (-w0) % m
+            cl, cg = (blk.convl2l.in_channels, blk.global_in_num) if blk is not None else (0, 0)
+            out.append(((1, cl, hp // f, wp // f), (1, cg, hp // f, wp // f), (h0, w0)))
+        return out
+
+    def native_ok(self, h: int, w: int) -> bool:
+        """Every scale of an (h, w) input has a native step program (else the group runs ``refine_predict``)."""
+        from . import engine as E
+        if os.environ.get("LAMA_B200_NATIVE_GRAD", "1") == "0":
+            return False
+        shapes = self.scale_shapes(h, w)
+        return bool(shapes) and all(E.refine_supported(self.generator, sl, sg, crop) for sl, sg, crop in shapes)
+
+    @staticmethod
+    def program_kind(scale: int, crop: Tuple[int, int]) -> str:
+        """The lowest scale (index 0) runs one forward; every other scale a step program."""
+        return "generator_rear" if scale == 0 else f"generator_refine:{crop[0]}x{crop[1]}"
+
+    def per_image_bytes(self, h: int, w: int) -> int:
+        """Pooled device bytes of the one-image programs of every scale of an (h, w) input (a batch keeps all of them
+        alive, so that the next batch of its size reuses their captured graphs)."""
+        from . import engine as E
+        total = 0
+        for s, (sl, sg, crop) in enumerate(self.scale_shapes(h, w)):
+            with torch.no_grad():
+                prog = E.build_module_program(self.generator, self.program_kind(s, crop), (sl, sg), E.default_math())
+            total += E.program_storage_bytes(prog)
+        return total
+
+    # -- execution
+    def _make_lane(self, kind: str, sl, sg, crop):
+        if kind == "generator_rear":
+            return _ForwardLane(self.generator, sl, sg, self.device)
+        return _StepLane(self.generator, sl, sg, crop, self.kw["lr"], self.device, self._graphs)
+
+    def _lane(self, b: int, scale: int, sl, sg, crop):
+        """The lane of scale ``scale`` at batch size ``b``.  Lanes of another batch size are released first: only one
+        batch's programs are alive at a time, which is what the batch plan budgets for."""
+        key = (b, sl[1:], sg[1:], crop)
+        if any(k[0] != b for k in self._lanes):
+            self._lanes.clear()
+            torch.cuda.empty_cache()
+        lane = self._lanes.get(key)
+        if lane is None:
+            sl, sg = (b,) + tuple(sl[1:]), (b,) + tuple(sg[1:])
+            lane = self._make_lane(self.program_kind(scale, crop), sl, sg, crop)
+            self._lanes[key] = lane
+        return lane
+
+    def _refine_batch(self, images: List[torch.Tensor], masks: List[torch.Tensor]) -> torch.Tensor:
+        """Equally sized (1,3,h,w) / (1,1,h,w) CPU images and masks -> (B,3,h',w') refined results on the device."""
+        kw, dev = self.kw, self.device
+        pyr = [image_mask_pyramid(im, mk, kw["min_side"], kw["max_scales"], kw["px_budget"])
+               for im, mk in zip(images, masks)]
+        ekernel = torch.from_numpy(ellipse_kernel(15)).float().to(dev)
+        shapes = self.scale_shapes(images[0].shape[2], images[0].shape[3])
+        result = None
+        for s, (sl, sg, crop) in enumerate(shapes):
+            im = torch.cat([_pad_to_modulo(p[0][s], kw["modulo"]) for p in pyr]).to(dev)
+            mk = torch.cat([_pad_to_modulo(p[1][s], kw["modulo"]) for p in pyr]).to(dev)
+            mk = (mk >= 1e-8).to(mk.dtype)
+            with torch.no_grad():
+                z1, z2 = self.front(torch.cat([im * (1 - mk), mk], dim=1))
+            lane = self._lane(len(images), s, sl, sg, crop)
+            h0, w0 = crop
+            consts = dict(image=im, mask=mk)
+            n_steps = 0
+            if result is not None:
+                md = pyrdown_mask(mk[:, :, :h0, :w0], blur_mask=False, round_up=False)
+                md = erode_mask(md, ekernel)
+                n = torch.stack([3 * (mk < 1e-8).sum((1, 2, 3)), 3 * (md >= 1e-8).sum((1, 2, 3))], 1).double()
+                inv = torch.where(n > 0, 1.0 / n.clamp_min(1), torch.zeros_like(n)).float()
+                consts.update(ref=result, md=md, inv=inv)
+                n_steps = kw["n_iters"] - 1
+            pred = lane.run(z1, z2, consts, n_steps)
+            result = (mk * pred + (1 - mk) * im)[:, :, :h0, :w0]
+        return result
+
+    def refine(self, images: Sequence[torch.Tensor], masks: Sequence[torch.Tensor]) -> List[torch.Tensor]:
+        """Float entry point: images (3,H,W) in [0,1] and masks (1,H,W) (mask / 255, not thresholded, as the
+        reference's dataset delivers them) on the CPU -> refined (3,H',W') float32 CPU tensors in input order."""
+        images = [im.float().cpu()[None] for im in images]
+        masks = [mk.float().cpu()[None] for mk in masks]
+        from .predict import BatchedInpainter
+        out: List[Optional[torch.Tensor]] = [None] * len(images)
+        for hw, idx in BatchedInpainter.plan([im.shape[2:] for im in images], self.max_batch):
+            if not self.native_ok(*hw):
+                for i in idx:
+                    out[i] = refine_predict(images[i], masks[i], self.generator, device=self.device, **self.kw)[0]
+                continue
+            if self._size != hw:                   # a new size: the previous size's step programs are done
+                self._lanes.clear()
+                torch.cuda.empty_cache()
+                budget = self.mem_budget
+                if budget is None:
+                    budget = int(0.7 * torch.cuda.mem_get_info(self.device)[0])
+                self._size, self._per_image, self._budget = hw, self.per_image_bytes(*hw), budget
+            for part in self.plan_batches(idx, self._per_image, self._budget, self.max_batch):
+                res = self._refine_batch([images[i] for i in part], [masks[i] for i in part]).cpu()
+                for j, i in enumerate(part):
+                    out[i] = res[j]
+        return out  # type: ignore[return-value]
+
+    def inpaint(self, items) -> List[np.ndarray]:
+        """items: (image HxWx3 uint8 RGB, mask HxW uint8) -> refined images HxWx3 uint8 in input order
+        (bin/predict.py:92: ``np.clip(x * 255, 0, 255).astype('uint8')``)."""
+        items = list(items)
+        for im, mk in items:
+            if im.dtype != np.uint8 or mk.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != 3 \
+                    or mk.shape != im.shape[:2]:
+                raise ValueError("expected (HxWx3 uint8 image, HxW uint8 mask) pairs")
+        imgs = [torch.from_numpy(np.ascontiguousarray(im)).permute(2, 0, 1).float() / 255 for im, _ in items]
+        msks = [torch.from_numpy(np.ascontiguousarray(mk))[None].float() / 255 for _, mk in items]
+        return [to_uint8(r) for r in self.refine(imgs, msks)]
+
+
+def to_uint8(x: torch.Tensor) -> np.ndarray:
+    """(3,H,W) float -> HxWx3 uint8 as bin/predict.py:92 writes it."""
+    return np.clip(x.permute(1, 2, 0).numpy() * 255, 0, 255).astype("uint8")
