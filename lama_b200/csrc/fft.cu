@@ -362,9 +362,9 @@ int check_fft_shapes(const ffcb_tensor* real, const ffcb_tensor* spec, const cha
 
 // fused whole-plane path (fft_plane.cu)
 bool plane64_eligible(const ffcb_tensor* real);
+bool plane64_inv_eligible(const ffcb_tensor* spec, const ffcb_tensor* residual, const ffcb_tensor* out);
 int rfft2_plane64(const ffcb_tensor* in, const ffcb_tensor* spec, cudaStream_t stream);
 int irfft2_plane64(const ffcb_tensor* spec, const ffcb_tensor* residual, const ffcb_tensor* out, cudaStream_t stream);
-int inv_plane_variant();
 // channel-group planar plane kernels (fft_plane_cg.cu)
 bool plane64_cg_fwd_eligible(const ffcb_tensor* in, const ffcb_tensor* spec);
 bool plane64_cg_inv_eligible(const ffcb_tensor* spec, const ffcb_tensor* residual, const ffcb_tensor* out);
@@ -440,12 +440,9 @@ int irfft2(const ffcb_tensor* spec, const ffcb_tensor* residual, const ffcb_tens
                  "residual and a split-bf16 cg=8 or float32 cg=4 output");
     return irfft2_plane64_cg(spec, residual, out, stream);
   }
-  // FFCB_FFT_INV_PLANE: 0 = two-pass kernels, 1 / 2 = first-revision plane kernels (slower than two-pass),
-  // 3 = second revision; irfft2_plane64 returns 1 when the chosen variant does not apply to these views
-  if (plane64_eligible(out) && inv_plane_variant() != 0 && !getenv("FFCB_FFT_TWO_PASS")) {
-    rc = irfft2_plane64(spec, residual, out, stream);
-    if (rc <= 0) return rc;
-  }
+  // views the plane kernel cannot take with 16-byte vector accesses run the two-pass kernels below
+  if (plane64_eligible(out) && plane64_inv_eligible(spec, residual, out) && !getenv("FFCB_FFT_TWO_PASS"))
+    return irfft2_plane64(spec, residual, out, stream);
   const View vspec = make_view(*spec), vout = make_view(*out);
   float2* w2 = reinterpret_cast<float2*>(ws);
   const int cblocks = (out->C + kLanes - 1) / kLanes;

@@ -344,64 +344,6 @@ FFCB_HD void plane64_col(Load&& ld, Store&& st) {
   for (int k = 0; k < 64; ++k) st(k, v[fft64_at(k)]);
 }
 
-// The DC (kx = 0) and Nyquist (kx = 32) columns are special: after the real row transforms they are REAL
-// (forward), and the C2R rule only uses the REAL part of their H-inverse (inverse).  Both therefore go
-// through one complex 64-point transform (two-for-one again), which makes the column phase exactly
-// 31 + 1 = 32 transforms per channel — the same 256 threads as the 32 row pairs.
-// Column transforms written as ONE instruction stream for both kinds of task (`packed` selects values,
-// only single loads / stores are predicated): the eight packed tasks of a CTA share a warp with 24 ordinary
-// columns, and a divergent branch around a whole 64-point transform would double that warp's critical path.
-//   ldA(y): column value (ordinary task) or DC column value (packed);  ldN(y): Nyquist column value (packed only)
-template <class LoadA, class LoadN, class StoreA, class StoreN>
-FFCB_HD void plane64_col_fwd_any(bool packed, LoadA&& ldA, LoadN&& ldN, StoreA&& stA, StoreN&& stN) {
-  float2 v[64];
-#pragma unroll
-  for (int n = 0; n < 64; ++n) {
-    const float2 a = ldA(n);
-    float2 q = make_float2(0.f, 0.f);
-    if (packed) q = ldN(n);
-    v[n] = packed ? make_float2(a.x, q.x) : a;           // DC / Nyquist columns are real after the row pass
-  }
-  fft64_regs<false>(v);
-#pragma unroll
-  for (int k = 0; k < 64; ++k) {
-    const float2 wk = v[fft64_at(k)], wm = v[fft64_at((64 - k) & 63)];
-    const float2 x0 = make_float2(0.5f * (wk.x + wm.x), 0.5f * (wk.y - wm.y));
-    const float2 x32 = make_float2(0.5f * (wk.y + wm.y), -0.5f * (wk.x - wm.x));
-    stA(k, packed ? x0 : wk);
-    if (packed) stN(k, x32);
-  }
-}
-
-template <class LoadA, class LoadN, class StoreA, class StoreN>
-FFCB_HD void plane64_col_inv_any(bool packed, LoadA&& ldA, LoadN&& ldN, StoreA&& stA, StoreN&& stN) {
-  float2 v[64];
-#pragma unroll
-  for (int n = 0; n < 64; ++n) v[n] = ldA(n);
-  // packed: v[k] <- H0[k] + i H32[k] with H = Hermitian part (its inverse transform is Re(ifft(Z)))
-#pragma unroll
-  for (int k = 0; k <= 32; ++k) {
-    const int m = (64 - k) & 63;
-    const float2 a = v[k], b = v[m];
-    float2 c = make_float2(0.f, 0.f), d = make_float2(0.f, 0.f);
-    if (packed) {
-      c = ldN(k);
-      d = (m != k) ? ldN(m) : c;
-    }
-    const float2 h0 = make_float2(0.5f * (a.x + b.x), 0.5f * (a.y - b.y));
-    const float2 h32 = make_float2(0.5f * (c.x + d.x), 0.5f * (c.y - d.y));
-    v[k] = packed ? make_float2(h0.x - h32.y, h0.y + h32.x) : a;
-    if (m != k) v[m] = packed ? make_float2(h0.x + h32.y, h32.x - h0.y) : b;
-  }
-  fft64_regs<true>(v);
-#pragma unroll
-  for (int n = 0; n < 64; ++n) {
-    const float2 z = v[fft64_at(n)];
-    stA(n, packed ? make_float2(z.x, 0.f) : z);
-    if (packed) stN(n, make_float2(z.y, 0.f));
-  }
-}
-
 template <class Load, class Store>
 FFCB_HD void plane64_rows_inv(Load&& ld, Store&& st) {
   float2 v[64];
@@ -428,7 +370,7 @@ FFCB_HD void plane64_rows_inv(Load&& ld, Store&& st) {
   }
 }
 
-// Inverse plane kernel, second revision (fft_plane.cu: irfft2_plane64_v2_kernel): after the C2R row transforms the
+// Inverse plane kernel (fft_plane.cu: irfft2_plane64_v2_kernel): after the C2R row transforms the
 // real results of row r are staged IN PLACE of that row's half spectrum (S row = 268 float2 = 536 floats >= 64 px x
 // 8 channels), channels-last, so that the epilogue moves whole pixels (8 channels = 32 bytes) with vector accesses.
 constexpr int kP64Pitch = 33 * 8 + 4;        // float2 per S row of the 8-channel plane kernels

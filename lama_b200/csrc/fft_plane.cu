@@ -1,48 +1,40 @@
-// Fused 2-D real FFT pair for 64x64 planes (the bottleneck of 512x512 images): one CTA transforms the
-// whole plane of 8 channels, so the half-spectrum intermediate lives in shared memory instead of a
-// global workspace (halves the HBM traffic of ffcb_rfft2 / ffcb_irfft2 and removes two launches).
+// Fused 2-D real FFT pair for 64x64 channels-last planes (the bottleneck of 512x512 images): one CTA transforms the
+// whole plane of 8 channels, so the half-spectrum intermediate lives in shared memory instead of a global workspace
+// (halves the HBM traffic of ffcb_rfft2 / ffcb_irfft2 and removes two launches).
 //
-// Every 64-point transform is held in the registers of ONE thread (fft64_regs: unrolled 8x8 Cooley-Tukey
-// with compile-time twiddles) — no shuffles, no shared-memory butterflies, one barrier per plane:
-//   forward : 256 threads = 8 channels x 32 row pairs (two-for-one real rows)  -> S[y][kx][c] -> barrier ->
-//             8 channels x (31 complex columns + 1 packed DC/Nyquist pair) -> spectrum (Re/Im interleaved, scaled)
-//   inverse : columns first (all 33, complex), barrier, then C2R rows (+ residual).
-// smem: S[64][P] float2 with row pitch P = 33*8 + 4 (the +4 spreads the four row-pair groups of a warp
-// over both halves of the banks).  Lanes: 8 consecutive channels (32 B of a pixel) x 4 rows/columns.
+// Every 64-point transform is held in the registers of ONE thread (fft64_regs: unrolled 8x8 Cooley-Tukey with
+// compile-time twiddles) — no shuffles, no shared-memory butterflies, one barrier per plane.  288 threads:
+//   forward : 256 threads = 8 channels x 32 row pairs (two-for-one real rows) -> S[y][kx][c] -> barrier ->
+//             264 threads = 8 channels x 33 complex columns -> spectrum (Re/Im interleaved, scaled; float32 or split
+//             bf16, chosen per store)
+//   inverse : 264 column tasks (complex, along H) -> S -> barrier -> 256 row-pair tasks (C2R along W), results staged
+//             channels-last in place of their rows -> whole-pixel vector epilogue (+ residual).  It takes a float32
+//             spectrum and residual and 16-byte aligned views (plane64_inv_eligible); fft.cu sends every other view
+//             to the two-pass kernels.
+// smem: S[64][kP64Pitch] float2, row pitch 33*8 + 4 (the +4 spreads the four row-pair groups of a warp over both
+// halves of the banks), 137 KB: one CTA per SM.  Lanes: 8 consecutive channels (32 B of a pixel) x 4 rows/columns.
 #include <stdint.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 #include "fft_core.cuh"
 
 namespace ffcb {
-int inv_plane_variant();   // FFCB_FFT_INV_PLANE (defined with the dispatchers at the end of this file)
 namespace {
 
 using namespace fftc;
 constexpr int PN = 64, PWF = 33;
-// Channels per CTA (PCH): 8 = one CTA per SM (137 KB of shared memory), lanes cover one full 32-byte sector of a
-// pixel; 4 = 69 KB, two CTAs per SM so that one CTA's load / store phases overlap the other's transforms
-// (FFCB_FFT_PLANE_CH=4, an experiment of round 1 — half-sector accesses, the sibling CTA picks up the other half
-// from L2).  The row pitch keeps the row-phase stores of a half-warp on 32 distinct banks: 4*P mod 32 = 128 / PCH.
-template <int PCH> struct PlaneCfg {
-  static constexpr int pitch = PWF * PCH + (PCH == 8 ? 4 : 2);
-  static constexpr int row_threads = 32 * PCH;                       // PCH channels x 32 row pairs
-  static constexpr int col_threads = (PWF * PCH + 31) / 32 * 32;     // PCH channels x 33 columns, whole warps
-  static constexpr size_t smem = sizeof(float2) * PN * pitch;
-  static constexpr int ctas_per_sm = PCH == 8 ? 1 : 2;
-};
+constexpr int PCH = 8;                                       // channels per CTA
+constexpr int kThreads = (PWF * PCH + 31) / 32 * 32;         // 33 x 8 column tasks, whole warps
+constexpr size_t kSmem = sizeof(float2) * PN * kP64Pitch;
 
-// Forward: rows by the first 32*PCH threads, the 33 x PCH column tasks by the first 33*PCH (for PCH = 8 chosen
-// over the packed 256-thread variant: fewer registers per thread, and one more warp to hide latency).
-template <int PCH, int OCC>
-__global__ void __launch_bounds__(PlaneCfg<PCH>::col_threads, OCC)
-rfft2_plane64_kernel(View in, View spec, float scale) {
+// Rows by the first 32*PCH threads, the 33 x PCH column tasks by the first 33*PCH (chosen over packing the DC and
+// Nyquist columns into one transform on 256 threads: fewer registers per thread, and one more warp to hide latency).
+__global__ void __launch_bounds__(kThreads, 1) rfft2_plane64_kernel(View in, View spec, float scale) {
   extern __shared__ float2 S[];
-  constexpr int PPITCH = PlaneCfg<PCH>::pitch;
+  constexpr int PPITCH = kP64Pitch;
   const int tid = threadIdx.x, c = tid % PCH, g = tid / PCH;
   const int ch = blockIdx.x * PCH + c, b = blockIdx.y;
-  if (tid < PlaneCfg<PCH>::row_threads) {   // g = row pair
+  if (tid < 32 * PCH) {   // g = row pair
     const long long r0 = pix_off(in, b, 2 * g, 0) + ch, r1 = r0 + in.sy;
     plane64_rows_fwd(
         [&](int n) { return make_float2(load1(in, r0 + n * in.sx), load1(in, r1 + n * in.sx)); },
@@ -73,106 +65,7 @@ rfft2_plane64_kernel(View in, View spec, float scale) {
   }
 }
 
-// Forward, second revision (default for float32 inputs).  Same algorithm and thread mapping; the differences are in
-// what surrounds the arithmetic (a third of the first revision's instruction body is 64-bit address arithmetic and
-// every access carries both format branches):
-//   * the spectrum format is a template parameter (one store path compiled in, no branch per store),
-//   * the CTA's base pointers are uniform (blockIdx-only) and every thread addresses with 32-bit offsets.
-template <int PCH, bool SPLIT>
-__global__ void __launch_bounds__(PlaneCfg<PCH>::col_threads, 1)
-rfft2_plane64_v2_kernel(const float* __restrict__ in_ptr, long long in_sb, unsigned in_sy, unsigned in_sx,
-                        void* __restrict__ spec_ptr, long long spec_sb, unsigned spec_sy, unsigned spec_sx,
-                        long long spec_lo, float scale) {
-  extern __shared__ float2 S[];
-  constexpr int PPITCH = PlaneCfg<PCH>::pitch;
-  const int tid = threadIdx.x, c = tid % PCH, g = tid / PCH;
-  if (tid < PlaneCfg<PCH>::row_threads) {   // g = row pair
-    const float* __restrict__ inb = in_ptr + (long long)blockIdx.y * in_sb + blockIdx.x * PCH;
-    const unsigned o0 = 2u * g * in_sy + c;
-    plane64_rows_fwd(
-        [&](int n) {
-          const unsigned o = o0 + (unsigned)n * in_sx;
-          return make_float2(__ldg(inb + o), __ldg(inb + o + in_sy));
-        },
-        [&](int k, float2 a, float2 bb) {
-          S[(2 * g) * PPITCH + k * PCH + c] = a;
-          S[(2 * g + 1) * PPITCH + k * PCH + c] = bb;
-        });
-  }
-  __syncthreads();
-  if (tid < PWF * PCH) {   // g = kx
-    const unsigned o0 = (unsigned)g * spec_sx + 2u * c;
-    const long long cta = (long long)blockIdx.y * spec_sb + 2 * blockIdx.x * PCH;
-    if constexpr (SPLIT) {
-      unsigned short* __restrict__ hi = reinterpret_cast<unsigned short*>(spec_ptr) + cta;
-      unsigned short* __restrict__ lo = hi + spec_lo;
-      plane64_col<false>(
-          [&](int y) { return S[y * PPITCH + g * PCH + c]; },
-          [&](int ky, float2 z) {
-            const unsigned o = o0 + (unsigned)ky * spec_sy;
-            __nv_bfloat16 h0, l0, h1, l1;
-            split_bf16(z.x * scale, h0, l0);
-            split_bf16(z.y * scale, h1, l1);
-            *reinterpret_cast<unsigned*>(hi + o) = pack_bf16(h0, h1);
-            *reinterpret_cast<unsigned*>(lo + o) = pack_bf16(l0, l1);
-          });
-    } else {
-      float* __restrict__ sp = reinterpret_cast<float*>(spec_ptr) + cta;
-      plane64_col<false>(
-          [&](int y) { return S[y * PPITCH + g * PCH + c]; },
-          [&](int ky, float2 z) {
-            const unsigned o = o0 + (unsigned)ky * spec_sy;
-            *reinterpret_cast<float2*>(sp + o) = make_float2(z.x * scale, z.y * scale);
-          });
-    }
-  }
-}
-
-template <int PCH>
-__global__ void __launch_bounds__(PlaneCfg<PCH>::row_threads, PlaneCfg<PCH>::ctas_per_sm)
-irfft2_plane64_kernel(View spec, View res, View out, float scale) {
-  extern __shared__ float2 S[];
-  constexpr int PPITCH = PlaneCfg<PCH>::pitch;
-  const int tid = threadIdx.x, c = tid % PCH, g = tid / PCH;
-  const int ch = blockIdx.x * PCH + c, b = blockIdx.y;
-  auto get = [&](long long o) {
-    if (spec.fmt == FFCB_F32) return __ldg(reinterpret_cast<const float2*>(reinterpret_cast<const float*>(spec.ptr) + o));
-    return make_float2(load1(spec, o), load1(spec, o + 1));
-  };
-  const long long o0 = pix_off(spec, b, 0, 0) + 2 * ch;
-  const bool packed = g == 0;
-  plane64_col_inv_any(
-      packed, [&](int ky) { return get(o0 + ky * spec.sy + g * spec.sx); },
-      [&](int ky) { return get(o0 + ky * spec.sy + 32 * spec.sx); },
-      [&](int y, float2 z) { S[y * PPITCH + g * PCH + c] = z; },
-      [&](int y, float2 z) { S[y * PPITCH + 32 * PCH + c] = z; });
-  __syncthreads();
-  {   // g = row pair: C2R along W
-    const long long r0 = pix_off(out, b, 2 * g, 0) + ch, r1 = r0 + out.sy;
-    const bool has_res = res.ptr != nullptr;
-    const long long q0 = has_res ? pix_off(res, b, 2 * g, 0) + ch : 0, q1 = q0 + res.sy;
-    plane64_rows_inv(
-        [&](int k, float2& x1, float2& x2) {
-          x1 = S[(2 * g) * PPITCH + k * PCH + c];
-          x2 = S[(2 * g + 1) * PPITCH + k * PCH + c];
-        },
-        [&](int n0, const float2* zb) {
-          float ra[16], rb[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            ra[j] = has_res ? load1(res, q0 + (n0 + j) * res.sx) : 0.f;
-            rb[j] = has_res ? load1(res, q1 + (n0 + j) * res.sx) : 0.f;
-          }
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            store1(out, r0 + (n0 + j) * out.sx, fmaf(zb[j].x, scale, ra[j]));
-            store1(out, r1 + (n0 + j) * out.sx, fmaf(zb[j].y, scale, rb[j]));
-          }
-        });
-  }
-}
-
-// Inverse, second revision (FFCB_FFT_INV_PLANE=3): the one-task-per-column variant below with
+// Inverse: one task per column, then C2R rows, with
 //   * formats as template parameters (float32 spectrum / residual in; float32 or split-bf16 out),
 //   * uniform CTA base pointers + 32-bit in-plane offsets,
 //   * a channels-last epilogue: row results are staged in place of the row's half spectrum and leave the SM as
@@ -186,10 +79,9 @@ struct PlaneInvArgs {
 };
 
 template <bool HAS_RES, bool OUT_SPLIT>
-__global__ void __launch_bounds__(PlaneCfg<8>::col_threads, 1) irfft2_plane64_v2_kernel(PlaneInvArgs a) {
+__global__ void __launch_bounds__(kThreads, 1) irfft2_plane64_v2_kernel(PlaneInvArgs a) {
   extern __shared__ float2 S[];
-  constexpr int PPITCH = PlaneCfg<8>::pitch;
-  static_assert(PPITCH == kP64Pitch, "staging indices assume the 8-channel pitch");
+  constexpr int PPITCH = kP64Pitch;
   const int tid = threadIdx.x, c = tid & 7, g = tid >> 3;
   if (tid < PWF * 8) {   // g = kx: inverse transform along H of one (column, channel)
     const float* __restrict__ sp = a.spec + (long long)blockIdx.y * a.spec_sb + 2 * blockIdx.x * 8;
@@ -253,126 +145,10 @@ __global__ void __launch_bounds__(PlaneCfg<8>::col_threads, 1) irfft2_plane64_v2
   }
 }
 
-// Inverse, 9-warp variant (FFCB_FFT_INV_PLANE=2): 264 independent column tasks (no packing), then 256 row tasks.
-template <int PCH>
-__global__ void __launch_bounds__(PlaneCfg<PCH>::col_threads, PlaneCfg<PCH>::ctas_per_sm)
-irfft2_plane64_9w_kernel(View spec, View res, View out, float scale) {
-  extern __shared__ float2 S[];
-  constexpr int PPITCH = PlaneCfg<PCH>::pitch;
-  const int tid = threadIdx.x, c = tid % PCH, g = tid / PCH;
-  const int ch = blockIdx.x * PCH + c, b = blockIdx.y;
-  if (tid < PWF * PCH) {   // g = kx
-    const long long o0 = pix_off(spec, b, 0, g) + 2 * ch;
-    plane64_col<true>(
-        [&](int ky) {
-          const long long o = o0 + ky * spec.sy;
-          if (spec.fmt == FFCB_F32) return __ldg(reinterpret_cast<const float2*>(reinterpret_cast<const float*>(spec.ptr) + o));
-          return make_float2(load1(spec, o), load1(spec, o + 1));
-        },
-        [&](int y, float2 z) { S[y * PPITCH + g * PCH + c] = z; });
-  }
-  __syncthreads();
-  if (tid < PlaneCfg<PCH>::row_threads) {   // g = row pair
-    const long long r0 = pix_off(out, b, 2 * g, 0) + ch, r1 = r0 + out.sy;
-    const bool has_res = res.ptr != nullptr;
-    const long long q0 = has_res ? pix_off(res, b, 2 * g, 0) + ch : 0, q1 = q0 + res.sy;
-    plane64_rows_inv(
-        [&](int k, float2& x1, float2& x2) {
-          x1 = S[(2 * g) * PPITCH + k * PCH + c];
-          x2 = S[(2 * g + 1) * PPITCH + k * PCH + c];
-        },
-        [&](int n0, const float2* zb) {
-          float ra[16], rb[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            ra[j] = has_res ? load1(res, q0 + (n0 + j) * res.sx) : 0.f;
-            rb[j] = has_res ? load1(res, q1 + (n0 + j) * res.sx) : 0.f;
-          }
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            store1(out, r0 + (n0 + j) * out.sx, fmaf(zb[j].x, scale, ra[j]));
-            store1(out, r1 + (n0 + j) * out.sx, fmaf(zb[j].y, scale, rb[j]));
-          }
-        });
-  }
-}
-
-int plane_channels() {
-  const char* e = getenv("FFCB_FFT_PLANE_CH");
-  return (e && atoi(e) == 4) ? 4 : 8;
-}
-
-template <int PCH, int OCC>
-int launch_fwd(const ffcb_tensor* in, const ffcb_tensor* spec, cudaStream_t stream) {
-  using Cfg = PlaneCfg<PCH>;
-  FFCB_CUDA(cudaFuncSetAttribute(rfft2_plane64_kernel<PCH, OCC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::smem));
-  dim3 grid(in->C / PCH, in->B);
-  rfft2_plane64_kernel<PCH, OCC><<<grid, Cfg::col_threads, Cfg::smem, stream>>>(make_view(*in), make_view(*spec), 1.0f / 64.0f);
-  FFCB_LAUNCH_CHECK("rfft2_plane64_kernel");
-  return FFCB_OK;
-}
-
-template <int PCH>
-int launch_inv(const ffcb_tensor* spec, const ffcb_tensor* residual, const ffcb_tensor* out, cudaStream_t stream) {
-  using Cfg = PlaneCfg<PCH>;
-  dim3 grid(out->C / PCH, out->B);
-  const View vres = (residual && residual->ptr) ? make_view(*residual) : null_view();
-  if (inv_plane_variant() == 2) {
-    FFCB_CUDA(cudaFuncSetAttribute(irfft2_plane64_9w_kernel<PCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::smem));
-    irfft2_plane64_9w_kernel<PCH><<<grid, Cfg::col_threads, Cfg::smem, stream>>>(make_view(*spec), vres, make_view(*out), 1.0f / 64.0f);
-    FFCB_LAUNCH_CHECK("irfft2_plane64_9w_kernel");
-    return FFCB_OK;
-  }
-  FFCB_CUDA(cudaFuncSetAttribute(irfft2_plane64_kernel<PCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::smem));
-  irfft2_plane64_kernel<PCH><<<grid, Cfg::row_threads, Cfg::smem, stream>>>(make_view(*spec), vres, make_view(*out), 1.0f / 64.0f);
-  FFCB_LAUNCH_CHECK("irfft2_plane64_kernel");
-  return FFCB_OK;
-}
-
-}  // namespace
-
-bool plane64_eligible(const ffcb_tensor* real) {
-  return real->H == PN && real->W == PN && real->C % 8 == 0 && real->B <= 65535;
-}
-
-template <bool SPLIT>
-int launch_fwd_v2(const ffcb_tensor* in, const ffcb_tensor* spec, cudaStream_t stream) {
-  using Cfg = PlaneCfg<8>;
-  FFCB_CUDA(cudaFuncSetAttribute(rfft2_plane64_v2_kernel<8, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::smem));
-  dim3 grid(in->C / 8, in->B);
-  rfft2_plane64_v2_kernel<8, SPLIT><<<grid, Cfg::col_threads, Cfg::smem, stream>>>(
-      reinterpret_cast<const float*>(in->ptr), in->sb, (unsigned)in->sy, (unsigned)in->sx, spec->ptr, spec->sb,
-      (unsigned)spec->sy, (unsigned)spec->sx, spec->lo_off, 1.0f / 64.0f);
-  FFCB_LAUNCH_CHECK("rfft2_plane64_v2_kernel");
-  return FFCB_OK;
-}
-
-constexpr int kDefaultFwdPlaneRevision = 1;      // until revision 2 has been validated / measured on the GPU
-
-// 32-bit in-plane offsets: 64 rows of either tensor must span fewer than 2^31 elements (always true on this path:
-// 64 x 64 pixels x at most a few thousand channels)
-bool fwd_v2_eligible(const ffcb_tensor* in, const ffcb_tensor* spec) {
-  const char* e = getenv("FFCB_FFT_PLANE_FWD");   // 1 = first revision, 2 = second
-  if ((e ? atoi(e) : kDefaultFwdPlaneRevision) != 2) return false;
-  return in->fmt == FFCB_F32 && plane_channels() == 8 && in->sy > 0 && in->sx > 0 && spec->sy > 0 && spec->sx > 0 &&
-         64 * in->sy < (1LL << 31) && 64 * spec->sy < (1LL << 31);
-}
-
-int rfft2_plane64(const ffcb_tensor* in, const ffcb_tensor* spec, cudaStream_t stream) {
-  if (fwd_v2_eligible(in, spec))
-    return spec->fmt == FFCB_BF16X2 ? launch_fwd_v2<true>(in, spec, stream) : launch_fwd_v2<false>(in, spec, stream);
-  if (plane_channels() == 4) {
-    const char* occ = getenv("FFCB_FFT_PLANE_OCC");      // 3: cap registers at 136 so that three CTAs share an SM
-    return (occ && atoi(occ) == 3) ? launch_fwd<4, 3>(in, spec, stream) : launch_fwd<4, 2>(in, spec, stream);
-  }
-  return launch_fwd<8, 1>(in, spec, stream);
-}
-
 template <bool HAS_RES, bool OUT_SPLIT>
-int launch_inv_v2(const PlaneInvArgs& a, dim3 grid, cudaStream_t stream) {
-  using Cfg = PlaneCfg<8>;
-  FFCB_CUDA(cudaFuncSetAttribute(irfft2_plane64_v2_kernel<HAS_RES, OUT_SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::smem));
-  irfft2_plane64_v2_kernel<HAS_RES, OUT_SPLIT><<<grid, Cfg::col_threads, Cfg::smem, stream>>>(a);
+int launch_inv(const PlaneInvArgs& a, dim3 grid, cudaStream_t stream) {
+  FFCB_CUDA(cudaFuncSetAttribute(irfft2_plane64_v2_kernel<HAS_RES, OUT_SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem));
+  irfft2_plane64_v2_kernel<HAS_RES, OUT_SPLIT><<<grid, kThreads, kSmem, stream>>>(a);
   FFCB_LAUNCH_CHECK("irfft2_plane64_v2_kernel");
   return FFCB_OK;
 }
@@ -383,39 +159,39 @@ bool vec_ok(const ffcb_tensor* t, int elems_per_16b) {   // 16-byte vector acces
          64 * t->sy < (1LL << 31);
 }
 
-bool inv_v2_eligible(const ffcb_tensor* spec, const ffcb_tensor* residual, const ffcb_tensor* out) {
-  if (plane_channels() != 8 || spec->fmt != FFCB_F32 || !vec_ok(spec, 2)) return false;
+}  // namespace
+
+bool plane64_eligible(const ffcb_tensor* real) {
+  return real->H == PN && real->W == PN && real->C % 8 == 0 && real->B <= 65535;
+}
+
+bool plane64_inv_eligible(const ffcb_tensor* spec, const ffcb_tensor* residual, const ffcb_tensor* out) {
+  if (spec->fmt != FFCB_F32 || !vec_ok(spec, 2)) return false;
   if (residual && residual->ptr && (residual->fmt != FFCB_F32 || !vec_ok(residual, 4))) return false;
   return vec_ok(out, out->fmt == FFCB_F32 ? 4 : 8);
 }
 
-// default: the second-revision plane kernel; 0 selects the two-pass kernels, which also take every view it cannot
-// handle
-constexpr int kDefaultInvPlaneVariant = 3;
-int inv_plane_variant() {
-  const char* e = getenv("FFCB_FFT_INV_PLANE");
-  if (!e || e[0] < '0' || e[0] > '3') return kDefaultInvPlaneVariant;
-  return e[0] - '0';
+int rfft2_plane64(const ffcb_tensor* in, const ffcb_tensor* spec, cudaStream_t stream) {
+  FFCB_CUDA(cudaFuncSetAttribute(rfft2_plane64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem));
+  dim3 grid(in->C / PCH, in->B);
+  rfft2_plane64_kernel<<<grid, kThreads, kSmem, stream>>>(make_view(*in), make_view(*spec), 1.0f / 64.0f);
+  FFCB_LAUNCH_CHECK("rfft2_plane64_kernel");
+  return FFCB_OK;
 }
 
-// returns FFCB_OK / a negative error, or 1 when the selected variant cannot handle these views (caller falls back)
+// views as plane64_eligible(out) && plane64_inv_eligible(spec, residual, out) accept
 int irfft2_plane64(const ffcb_tensor* spec, const ffcb_tensor* residual, const ffcb_tensor* out, cudaStream_t stream) {
-  const int variant_id = inv_plane_variant();
-  if (variant_id == 3) {
-    if (!inv_v2_eligible(spec, residual, out)) return 1;
-    const bool has_res = residual && residual->ptr;
-    PlaneInvArgs a;
-    a.spec = reinterpret_cast<const float*>(spec->ptr); a.spec_sb = spec->sb; a.spec_sy = (unsigned)spec->sy; a.spec_sx = (unsigned)spec->sx;
-    a.res = has_res ? reinterpret_cast<const float*>(residual->ptr) : nullptr;
-    a.res_sb = has_res ? residual->sb : 0; a.res_sy = has_res ? (unsigned)residual->sy : 0; a.res_sx = has_res ? (unsigned)residual->sx : 0;
-    a.out = out->ptr; a.out_sb = out->sb; a.out_sy = (unsigned)out->sy; a.out_sx = (unsigned)out->sx; a.out_lo = out->lo_off;
-    a.scale = 1.0f / 64.0f;
-    dim3 grid(out->C / 8, out->B);
-    const bool split = out->fmt == FFCB_BF16X2;
-    if (has_res) return split ? launch_inv_v2<true, true>(a, grid, stream) : launch_inv_v2<true, false>(a, grid, stream);
-    return split ? launch_inv_v2<false, true>(a, grid, stream) : launch_inv_v2<false, false>(a, grid, stream);
-  }
-  return plane_channels() == 4 ? launch_inv<4>(spec, residual, out, stream) : launch_inv<8>(spec, residual, out, stream);
+  const bool has_res = residual && residual->ptr;
+  PlaneInvArgs a;
+  a.spec = reinterpret_cast<const float*>(spec->ptr); a.spec_sb = spec->sb; a.spec_sy = (unsigned)spec->sy; a.spec_sx = (unsigned)spec->sx;
+  a.res = has_res ? reinterpret_cast<const float*>(residual->ptr) : nullptr;
+  a.res_sb = has_res ? residual->sb : 0; a.res_sy = has_res ? (unsigned)residual->sy : 0; a.res_sx = has_res ? (unsigned)residual->sx : 0;
+  a.out = out->ptr; a.out_sb = out->sb; a.out_sy = (unsigned)out->sy; a.out_sx = (unsigned)out->sx; a.out_lo = out->lo_off;
+  a.scale = 1.0f / 64.0f;
+  dim3 grid(out->C / PCH, out->B);
+  const bool split = out->fmt == FFCB_BF16X2;
+  if (has_res) return split ? launch_inv<true, true>(a, grid, stream) : launch_inv<true, false>(a, grid, stream);
+  return split ? launch_inv<false, true>(a, grid, stream) : launch_inv<false, false>(a, grid, stream);
 }
 
 }  // namespace ffcb

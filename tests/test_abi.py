@@ -63,10 +63,11 @@ def test_missing_library_is_loud(monkeypatch, tmp_path):
         _lib.get_lib()
 
 
-def test_host_emulation_of_fft_kernels(tmp_path):
+def test_host_emulation_of_fft_and_shipped_plane_kernels(tmp_path):
     """The FFT kernels' arithmetic (fft_core.cuh) compiled for the host and checked against a
     double-precision DFT for every supported size class (pow2 Stockham, direct DFT, runtime mixed-radix Stockham
-    plans for composite / prime-power / prime lengths, C2R rule, fused 64x64 plane functors)."""
+    plans for composite / prime-power / prime lengths, C2R rule), and the per-thread steps of the 64x64 plane pair as
+    rfft2_plane64_kernel / irfft2_plane64_v2_kernel run them."""
     exe = tmp_path / "fft_emul"
     subprocess.check_call(["g++", "-O2", "-std=c++17", "-I/usr/local/cuda/include",
                            os.path.join(ROOT, "tests", "host_emul", "fft_emul.cpp"), "-o", str(exe)])

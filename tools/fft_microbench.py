@@ -1,6 +1,6 @@
 """FFT microbenchmark (CUDA events on the launch stream, warm, inputs larger than... see below):
-  * the FourierUnit shape of the headline workload (B=32, C=192, 64x64 planes) under the plane-kernel variants
-    (FFCB_FFT_PLANE_CH / FFCB_FFT_PLANE_OCC / FFCB_FFT_INV_PLANE / FFCB_FFT_TWO_PASS), forward and inverse apart;
+  * the FourierUnit shape of the headline workload (B=32, C=192, 64x64 planes): the plane kernels against the
+    two-pass kernels (FFCB_FFT_TWO_PASS), forward and inverse apart;
   * planes without a compile-time plan (row f2): direct DFT vs runtime mixed-radix Stockham.
 Run on the GPU box:  python tools/fft_microbench.py  -> one JSON line per configuration."""
 import json
@@ -13,8 +13,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from lama_b200 import _lib as L          # noqa: E402
 from lama_b200 import engine as E        # noqa: E402
 
-KNOBS = ("FFCB_FFT_MIXED_RADIX", "FFCB_FFT_PLANE_CH", "FFCB_FFT_PLANE_OCC", "FFCB_FFT_INV_PLANE", "FFCB_FFT_TWO_PASS",
-         "FFCB_FFT_PLANE_FWD")
+KNOBS = ("FFCB_FFT_MIXED_RADIX", "FFCB_FFT_TWO_PASS")
 
 
 def time_ops(b, c, h, w, env, which, reps=10, spec_fmt_split=True, warm=3):
@@ -111,23 +110,13 @@ if __name__ == "__main__":
     if "--chain-planar-once" in sys.argv:   # one pass of the planar chain (for ncu captures)
         print(json.dumps(time_fu_chain(*fu, True, reps=1, warm=1)), flush=True)
         sys.exit(0)
-    if "--v2" in sys.argv:               # first vs second revision of the plane kernels at the headline shape
-        for env in [{"FFCB_FFT_PLANE_FWD": "1"}, {"FFCB_FFT_PLANE_FWD": "2"}]:
-            print(json.dumps(time_ops(*fu, env, "fwd", reps=20)), flush=True)
-        for env in [{"FFCB_FFT_INV_PLANE": "0"}, {"FFCB_FFT_INV_PLANE": "2"}, {"FFCB_FFT_INV_PLANE": "3"}]:
-            print(json.dumps(time_ops(*fu, env, "inv", reps=20)), flush=True)
-        sys.exit(0)
     if "--fu-only" in sys.argv:          # the shipped configuration only (for an ncu capture)
         print(json.dumps(time_ops(*fu, {}, "fwd", reps=1, warm=0)), flush=True)
         print(json.dumps(time_ops(*fu, {}, "inv", reps=1, warm=0)), flush=True)
         sys.exit(0)
-    for env in [{}, {"FFCB_FFT_PLANE_CH": "4"}, {"FFCB_FFT_PLANE_CH": "4", "FFCB_FFT_PLANE_OCC": "3"},
-                {"FFCB_FFT_TWO_PASS": "1"}]:
-        print(json.dumps(time_ops(*fu, env, "fwd")), flush=True)
-    for env in [{}, {"FFCB_FFT_INV_PLANE": "1"}, {"FFCB_FFT_INV_PLANE": "2"},
-                {"FFCB_FFT_INV_PLANE": "1", "FFCB_FFT_PLANE_CH": "4"},
-                {"FFCB_FFT_INV_PLANE": "2", "FFCB_FFT_PLANE_CH": "4"}]:
-        print(json.dumps(time_ops(*fu, env, "inv")), flush=True)
+    for which in ("fwd", "inv"):
+        for env in [{}, {"FFCB_FFT_TWO_PASS": "1"}]:
+            print(json.dumps(time_ops(*fu, env, which)), flush=True)
     for (h, w) in [(96, 128), (125, 188), (135, 240)]:
         for mixed in ("0", "1"):
             for which in ("fwd", "inv"):
