@@ -91,37 +91,107 @@ class TV:
         return (self.buf.H // 2, self.buf.W // 2) if self.phase else (self.buf.H, self.buf.W)
 
 
+@dataclass(frozen=True)
+class Ext:
+    """A program input or output named in a call's argument list.  The executor turns an output into its tensor's
+    pointer when it binds the call, and an input into a slot that ``CudaExecutor.bind_inputs`` patches."""
+    name: str
+
+
+OP_TYPES: List[type] = []       # every op record type (tests check that each one is fully declared)
+
+# What an op does to the reflected ring of a buffer it writes:
+STALE = "stale"          # the interior changes, the ring does not: insert_border_ops refreshes it before a ring read
+REWRITES = "rewrites"    # the op writes the ring from the new interior itself
+KEEPS = "keeps"          # the op sums reflected rings, so the output ring stays a reflection (ffcb_add)
+
+
+class Op:
+    """Base of the op records.  Each type declares, in one place, the fields holding the views it reads and writes
+    (``reads`` / ``writes``; a field may hold a view, None, or a list of views or of (view, int) pairs), its ring
+    effect on the buffers it writes and the reads that need a valid ring (``ring_in``), its FFT workspace and scratch,
+    and ``bind(ex)``: its one C-ABI call on executor ``ex`` as (call name, library function, argument list without the
+    trailing stream), or None."""
+    reads: Tuple[str, ...]          # every op type sets both
+    writes: Tuple[str, ...]
+    ring_in: Tuple[str, ...] = ()
+    ring = STALE
+
+    def __init_subclass__(cls, **kw):
+        super().__init_subclass__(**kw)
+        OP_TYPES.append(cls)
+
+    def _tvs(self, names) -> List[TV]:
+        flat = [x for v in (getattr(self, n) for n in names) for x in (v if isinstance(v, list) else [v])]
+        return [x[0] if isinstance(x, tuple) else x for x in flat if x is not None]     # (view, int) pairs: FoldOp
+
+    def views(self) -> Tuple[List[TV], List[TV]]:
+        """(views read, views written) — the basis of the buffer liveness analysis."""
+        return self._tvs(self.reads), self._tvs(self.writes)
+
+    def ring_reads(self) -> List[TV]:
+        return self._tvs(self.ring_in)
+
+    def ring_effect(self, prog) -> str:
+        return self.ring
+
+    def workspace_bytes(self) -> int:
+        return 0
+
+    def scratch_bytes(self) -> int:
+        """Device scratch the op's binding allocates besides the program's buffers."""
+        return 0
+
+
 @dataclass
-class ToNHWC:
+class ToNHWC(Op):
+    reads, writes = (), ("out",)
     src: str          # name of an external NCHW float tensor
     out: TV
 
+    def bind(self, ex):
+        return "ffcb_nchw_to_nhwc", ex.lib.ffcb_nchw_to_nhwc, [Ext(self.src), *ex.prog.inputs[self.src], ex.ref(self.out)]
+
 
 @dataclass
-class ToNCHW:
+class ToNCHW(Op):
+    reads, writes = ("inp",), ()
     inp: TV
     dst: str          # name of an external NCHW float output
 
+    def bind(self, ex):
+        return "ffcb_nhwc_to_nchw", ex.lib.ffcb_nhwc_to_nchw, [ex.ref(self.inp), Ext(self.dst)]
+
 
 @dataclass
-class StemOp:
+class StemOp(Op):
+    reads, writes = (), ("out",)
     src: str          # external NCHW input
     cin: int
     w: torch.Tensor   # [(ky*7+kx)*Cin + c][N]
     shift: torch.Tensor
     out: TV
 
+    def bind(self, ex):
+        return "ffcb_stem_conv7", ex.lib.ffcb_stem_conv7, [Ext(self.src), *ex.prog.inputs[self.src], ex.keep(self.w),
+                                                           ex.keep(self.shift), self.w.shape[1], ex.ref(self.out)]
+
 
 @dataclass
-class StemPackOp:
+class StemPackOp(Op):
     """NCHW float input -> reflect-padded NHWC8 image for the tensor-core stem (ffcb_stem_pack)."""
+    reads, writes = (), ("out",)
     src: str
     cin: int
     out: TV           # Buf (B, H+6, W+8, 8)
 
+    def bind(self, ex):
+        return "ffcb_stem_pack", ex.lib.ffcb_stem_pack, [Ext(self.src), *ex.prog.inputs[self.src], ex.ref(self.out)]
+
 
 @dataclass
-class HeadOp:
+class HeadOp(Op):
+    reads, writes = ("inp",), ()
     inp: TV
     w: torch.Tensor   # [N][49][C]
     bias: torch.Tensor
@@ -129,31 +199,46 @@ class HeadOp:
     act: int
     dst: str
 
+    def bind(self, ex):
+        return "ffcb_head_conv7", ex.lib.ffcb_head_conv7, [ex.ref(self.inp), ex.keep(self.w), ex.keep(self.bias),
+                                                           self.n_out, self.act, Ext(self.dst)]
+
 
 @dataclass
-class HeadGatherOp:
+class HeadGatherOp(Op):
     """y = act(bias + sum_kx q[.., reflect(x+kx-3), n*7+kx]) -> external NCHW output (ffcb_head_gather7)."""
+    reads, writes = ("q",), ()
     q: TV
     bias: torch.Tensor
     n_out: int
     act: int
     dst: str
 
+    def bind(self, ex):
+        return "ffcb_head_gather7", ex.lib.ffcb_head_gather7, [ex.ref(self.q), ex.keep(self.bias), self.n_out, self.act,
+                                                               Ext(self.dst)]
+
 
 @dataclass
-class StemPackU8Op:
+class StemPackU8Op(Op):
     """Decoded RGB bytes + mask bytes -> packed stem image (ffcb_stem_pack_u8): /255, symmetric pad to the
     modulo size, mask > 0, img * (1 - mask), cat(mask), ReflectionPad2d(3)."""
+    reads, writes = (), ("out",)
     img: str          # external uint8 (B, H0, W0, 3)
     mask: str         # external uint8 (B, H0, W0)
     h0: int
     w0: int
     out: TV           # Buf (B, H+6, W+8, 8)
 
+    def bind(self, ex):
+        return "ffcb_stem_pack_u8", ex.lib.ffcb_stem_pack_u8, [Ext(self.img), Ext(self.mask), ex.prog.inputs[self.img][0],
+                                                               self.h0, self.w0, ex.ref(self.out)]
+
 
 @dataclass
-class HeadGatherU8Op:
+class HeadGatherU8Op(Op):
     """ffcb_head_gather7_blend_u8: head gather + activation + blend with the input + crop + x255/clip/truncate."""
+    reads, writes = ("q",), ()
     q: TV
     bias: torch.Tensor
     act: int
@@ -163,9 +248,14 @@ class HeadGatherU8Op:
     w0: int
     dst: str          # external uint8 (B, H0, W0, 3)
 
+    def bind(self, ex):
+        return "ffcb_head_gather7_blend_u8", ex.lib.ffcb_head_gather7_blend_u8, [
+            ex.ref(self.q), ex.keep(self.bias), self.act, Ext(self.img), Ext(self.mask), self.h0, self.w0, Ext(self.dst)]
+
 
 @dataclass
-class ConvOp:
+class ConvOp(Op):
+    reads, writes, ring_in = ("ins", "addend"), ("out",), ("ins",)
     packed: P.PackedConv
     ins: List[Optional[TV]]
     out: TV
@@ -173,66 +263,125 @@ class ConvOp:
     addend_post: bool = False
     tag: str = ""
 
+    def ring_effect(self, prog):
+        return REWRITES if conv_writes_ring(prog, self) else STALE
+
+    def bind(self, ex):
+        d = L.ConvDesc()
+        pk = self.packed
+        d.inp[0] = ex.tensor(self.ins[0])
+        if self.ins[1] is not None:
+            d.inp[1] = ex.tensor(self.ins[1])
+        d.out = ex.tensor(self.out)
+        if self.addend is not None:
+            d.addend = ex.tensor(self.addend)
+        d.weight = ex.keep(pk.split_weights() if ex.prog.math == L.MATH_BF16X3 else pk.w_kn)
+        if pk.shift is not None:
+            d.shift = ex.keep(pk.shift)
+        d.n_out, d.stride, d.border, d.act = pk.n_out, pk.stride, pk.border, pk.act
+        d.nseg, d.math, d.addend_post = len(pk.segs), ex.prog.math, int(self.addend_post)
+        for i, s in enumerate(pk.segs):
+            d.seg[i] = L.KSeg(s.src, s.dy, s.dx, s.c0, s.nch)
+        return "ffcb_conv:" + self.tag, ex.lib.ffcb_conv, [ex.ref(d)]
+
 
 @dataclass
-class RfftOp:
+class RfftOp(Op):
+    reads, writes = ("inp",), ("spec",)
     inp: TV
     spec: TV
 
+    def workspace_bytes(self):
+        return 8 * self.inp.batch * self.inp.hw[0] * (self.inp.hw[1] // 2 + 1) * self.inp.channels
+
+    def bind(self, ex):
+        return "ffcb_rfft2", ex.lib.ffcb_rfft2, [ex.ref(self.inp), ex.ref(self.spec), ex.ws.data_ptr(), ex.ws_bytes]
+
 
 @dataclass
-class IrfftOp:
+class IrfftOp(Op):
+    reads, writes = ("spec", "residual"), ("out",)
     spec: TV
     residual: Optional[TV]
     out: TV
 
+    def workspace_bytes(self):
+        return 8 * self.out.batch * self.out.hw[0] * (self.out.hw[1] // 2 + 1) * self.out.channels
+
+    def bind(self, ex):
+        return "ffcb_irfft2", ex.lib.ffcb_irfft2, [ex.ref(self.spec), ex.ref(self.residual), ex.ref(self.out),
+                                                   ex.ws.data_ptr(), ex.ws_bytes]
+
 
 @dataclass
-class BorderOp:
+class BorderOp(Op):
     """(Re)build the reflected ring of a padded buffer after a producer that does not write it."""
+    reads, writes, ring = ("view",), ("view",), REWRITES
     view: TV
 
+    def bind(self, ex):
+        return "ffcb_fill_reflect_border", ex.lib.ffcb_fill_reflect_border, [ex.ref(self.view)]
+
 
 @dataclass
-class ReluBwdOp:
+class ReluBwdOp(Op):
     """out = dy * [y > 0] (ffcb_relu_bwd): ReLU backward with the forward activation."""
+    reads, writes = ("dy", "y"), ("out",)
     dy: TV
     y: TV
     out: TV
 
+    def bind(self, ex):
+        return "ffcb_relu_bwd", ex.lib.ffcb_relu_bwd, [ex.ref(self.dy), ex.ref(self.y), ex.ref(self.out)]
+
 
 @dataclass
-class FoldOp:
+class FoldOp(Op):
     """Adjoint of the 1-pixel reflect padding (ffcb_fold_reflect_border): gradient w.r.t. the padded plane ``gpad``
     (B,H+2,W+2,C) folded onto the interior, plus optional addends written as (view, first output channel)."""
+    reads, writes = ("gpad", "addends"), ("out",)
     gpad: TV
     addends: List[Tuple[TV, int]]
     out: TV
 
+    def bind(self, ex):
+        adds = [(ex.ref(tv), c0) for tv, c0 in self.addends] + [(None, 0)] * 2
+        return "ffcb_fold_reflect_border", ex.lib.ffcb_fold_reflect_border, [
+            ex.ref(self.gpad), adds[0][0], adds[0][1], adds[1][0], adds[1][1], ex.ref(self.out)]
+
 
 @dataclass
-class AddOp:
+class AddOp(Op):
     """out = a + b over the whole padded extent of three views of one geometry (ffcb_add); ``out`` may be ``a``."""
+    reads, writes, ring_in, ring = ("a", "b"), ("out",), ("a", "b"), KEEPS
     a: TV
     b: TV
     out: TV
 
+    def bind(self, ex):
+        return "ffcb_add", ex.lib.ffcb_add, [ex.ref(self.a), ex.ref(self.b), ex.ref(self.out)]
+
 
 @dataclass
-class HeadBwdOp:
+class HeadBwdOp(Op):
     """Adjoint of ReflectionPad2d(3) + 7x7 head + act, masked by the last up-sampling ReLU (ffcb_head_bwd7):
     out = [mask > 0] * Fold3(Conv7^T(act'(y) * dy)), with y / dy the external NCHW output and its gradient."""
+    reads, writes = ("mask",), ("out",)
     y: str            # external output of the forward part (the head's)
-    dy: str           # external NCHW input of the backward part
+    dy: str           # external NCHW gradient: an input of the backward part, or an output an earlier op writes
     w: torch.Tensor   # [N][49][C] (pack_head)
     n_out: int
     act: int
     mask: TV
     out: TV
 
+    def bind(self, ex):
+        return "ffcb_head_bwd7", ex.lib.ffcb_head_bwd7, [Ext(self.y), Ext(self.dy), *ex.prog.outputs[self.y],
+                                                         ex.keep(self.w), self.act, ex.ref(self.mask), ex.ref(self.out)]
+
 
 @dataclass
-class RefineLossOp:
+class RefineLossOp(Op):
     """Gradient of the refinement loss w.r.t. the prediction, and its two terms (ffcb_refine_l1_grad): every operand
     is an external NCHW tensor of the program — ``pred`` and the outputs ``grad`` / ``loss`` are program outputs, the
     rest per-scale inputs (image, mask, ref, md, inv = 1 / n per image and term)."""
@@ -248,11 +397,26 @@ class RefineLossOp:
     grad: str
     loss: str
     ref_numel: int        # B * C * (H0/2) * (W0/2): the kernel's low-resolution scratch
+    reads, writes = (), ()    # external tensors only
+
+    def scratch_bytes(self):
+        return 4 * self.ref_numel
+
+    def bind(self, ex):
+        work = ex.keep(torch.empty(self.ref_numel, dtype=torch.float32))
+        return "ffcb_refine_l1_grad", ex.lib.ffcb_refine_l1_grad, [
+            Ext(self.pred), Ext(self.image), Ext(self.mask), *ex.prog.outputs[self.pred], self.h0, self.w0,
+            Ext(self.ref), Ext(self.md), Ext(self.inv), ex.keep(self.taps.float()), work, Ext(self.grad), Ext(self.loss)]
 
 
 @dataclass
-class SplitOp:
+class SplitOp(Op):
     """Boundary between the forward and the backward part of a forward+backward program (no kernel)."""
+    reads, writes = (), ()
+
+    def bind(self, ex):
+        ex.split = len(ex.calls)
+        return None
 
 
 @dataclass
@@ -283,16 +447,7 @@ class Program:
         return b
 
     def fft_workspace_bytes(self) -> int:
-        need = 0
-        for op in self.ops:
-            if isinstance(op, RfftOp):
-                b, (h, w), c = op.inp.batch, op.inp.hw, op.inp.channels
-            elif isinstance(op, IrfftOp):
-                b, (h, w), c = op.out.batch, op.out.hw, op.out.channels
-            else:
-                continue
-            need = max(need, 8 * b * h * (w // 2 + 1) * c)
-        return need
+        return max((op.workspace_bytes() for op in self.ops), default=0)
 
 
 # ------------------------------------------------------------------------------- support predicates
@@ -1166,27 +1321,15 @@ def insert_border_ops(prog: Program):
     tensor map of the interior; layout conversions, the stem and the FFT kernels write pixels only).  Insert
     a BorderOp lazily: right before the first contraction that reads a buffer whose interior changed since
     its ring was last rebuilt.  For the in-place residual blocks that is one ring refresh per FFC_BN_ACT."""
-    out, dirty = [], {}
+    out, dirty = [], set()
     for op in prog.ops:
-        if isinstance(op, ConvOp):
-            for tv in op.ins:
-                if tv is not None and tv.buf.reflect_border and id(tv.buf) in dirty:
-                    out.append(BorderOp(TV(tv.buf)))
-                    del dirty[id(tv.buf)]
-        elif isinstance(op, AddOp):
-            # ffcb_add sums the rings too: its output ring is a reflection when both input rings are
-            for tv in (op.a, op.b):
-                if tv.buf.reflect_border and id(tv.buf) in dirty:
-                    out.append(BorderOp(TV(tv.buf)))
-                    del dirty[id(tv.buf)]
+        for tv in op.ring_reads():
+            if tv.buf.reflect_border and id(tv.buf) in dirty:
+                out.append(BorderOp(TV(tv.buf)))
+                dirty.discard(id(tv.buf))
         out.append(op)
-        wrote = None
-        if isinstance(op, (ToNHWC, StemOp, StemPackOp, StemPackU8Op, IrfftOp, ConvOp)):
-            wrote = op.out
-        elif isinstance(op, RfftOp):
-            wrote = op.spec
-        if wrote is not None and wrote.buf.reflect_border and not conv_writes_ring(prog, op):
-            dirty[id(wrote.buf)] = wrote.buf
+        if op.ring_effect(prog) == STALE:
+            dirty.update(id(tv.buf) for tv in op.views()[1] if tv.buf.reflect_border)
     prog.ops = out
 
 
@@ -1203,32 +1346,12 @@ def conv_writes_ring(prog: Program, op) -> bool:
 
 # ------------------------------------------------------------------------------------- executor
 def op_views(op) -> Tuple[List[TV], List[TV]]:
-    """(views read, views written) by one op of a program — the basis of the buffer liveness analysis."""
-    if isinstance(op, (ToNHWC, StemOp, StemPackOp, StemPackU8Op)):
-        return [], [op.out]
-    if isinstance(op, (ToNCHW, HeadOp)):
-        return [op.inp], []
-    if isinstance(op, (HeadGatherOp, HeadGatherU8Op)):
-        return [op.q], []
-    if isinstance(op, ConvOp):
-        return [t for t in op.ins if t is not None] + ([op.addend] if op.addend is not None else []), [op.out]
-    if isinstance(op, RfftOp):
-        return [op.inp], [op.spec]
-    if isinstance(op, IrfftOp):
-        return [op.spec] + ([op.residual] if op.residual is not None else []), [op.out]
-    if isinstance(op, BorderOp):
-        return [op.view], [op.view]
-    if isinstance(op, ReluBwdOp):
-        return [op.dy, op.y], [op.out]
-    if isinstance(op, FoldOp):
-        return [op.gpad] + [tv for tv, _c0 in op.addends], [op.out]
-    if isinstance(op, AddOp):
-        return [op.a, op.b], [op.out]
-    if isinstance(op, HeadBwdOp):
-        return [op.mask], [op.out]
-    if isinstance(op, (SplitOp, RefineLossOp)):         # RefineLossOp reads and writes external tensors only
-        return [], []
-    raise TypeError(op)
+    """(views read, views written) by one op of a program: ``op.views()``."""
+    return op.views()
+
+
+def op_scratch_bytes(op) -> int:
+    return op.scratch_bytes()
 
 
 def storage_key(b: Buf) -> tuple:
@@ -1245,13 +1368,6 @@ def storage_shape(b: Buf) -> Tuple[int, ...]:
     return (b.B, b.H + 2 * b.pad, b.W + 2 * b.pad, b.C)
 
 
-def op_scratch_bytes(op) -> int:
-    """Device scratch an op's binding allocates besides the program's buffers."""
-    if isinstance(op, RefineLossOp):
-        return 4 * op.ref_numel
-    return 0
-
-
 def program_storage_bytes(prog: Program) -> int:
     """Device bytes a ``CudaExecutor`` of ``prog`` allocates for activations, computed from the buffer shapes and
     storage slots before anything is allocated: the pooled buffers, the FFT workspace, the program's outputs and op
@@ -1264,7 +1380,7 @@ def program_storage_bytes(prog: Program) -> int:
             total += 4 * math.prod(storage_shape(b))           # float32, or two bfloat16 halves
     for name, shape in prog.outputs.items():
         total += math.prod(shape) * (1 if prog.dtypes.get(name, torch.float32) == torch.uint8 else 4)
-    return total + max(prog.fft_workspace_bytes(), 16) + sum(op_scratch_bytes(op) for op in prog.ops)
+    return total + max(prog.fft_workspace_bytes(), 16) + sum(op.scratch_bytes() for op in prog.ops)
 
 
 def assign_storage_slots(prog: Program) -> Dict[str, int]:
@@ -1278,7 +1394,7 @@ def assign_storage_slots(prog: Program) -> Dict[str, int]:
     first: Dict[str, int] = {}
     last: Dict[str, int] = {}
     for i, op in enumerate(prog.ops):
-        reads, writes = op_views(op)
+        reads, writes = op.views()
         for tv in reads + writes:
             first.setdefault(tv.buf.name, i)
             last[tv.buf.name] = i
@@ -1336,12 +1452,31 @@ class CudaExecutor:
                         for k, v in prog.outputs.items()}
         self._launches = None
         self._keep = []          # ctypes objects / tensors that must outlive the calls
-        self.calls = []          # (fn, args) with a trailing stream argument appended at run time
+        self.calls = []          # (name, fn, args) with a trailing stream argument appended at run time
         self.input_slots: Dict[str, List[Tuple[int, int]]] = {}   # input name -> [(call idx, arg idx)]
         self.split = None        # forward+backward programs: index of the first backward call (SplitOp)
         self.generation = 0      # bumped by every forward part: a stale backward must not read newer activations
+        assert not prog.inputs.keys() & prog.outputs.keys(), "a name is both a program input and a program output"
         for op in prog.ops:
-            self._bind(op)
+            call = op.bind(self)
+            if call is None:
+                continue
+            name, fn, args = call
+            for ai, a in enumerate(args):
+                if isinstance(a, Ext):
+                    if a.name in self.outputs:
+                        args[ai] = self.outputs[a.name].data_ptr()
+                    else:
+                        assert a.name in prog.inputs, f"{name} reads {a.name!r}, neither an input nor an output"
+                        self.input_slots.setdefault(a.name, []).append((len(self.calls), ai))
+                        args[ai] = None
+            self.calls.append((name, fn, args))
+        # part -> (first call, end, inputs its calls read); parts 0 / 1 exist for forward+backward programs
+        n = len(self.calls)
+        spans = {None: (0, n)} if self.split is None else {None: (0, n), 0: (0, self.split), 1: (self.split, n)}
+        self._parts = {p: (lo, hi, {n for n, sl in self.input_slots.items() if any(lo <= ci < hi for ci, _ in sl)})
+                       for p, (lo, hi) in spans.items()}
+        self._bound = set()      # inputs bound at least once
 
     # -- view construction
     def tensor(self, tv: TV) -> L.Tensor:
@@ -1406,176 +1541,59 @@ class CudaExecutor:
             t.W, t.C, t.window = b.W - tv.window, b.C * tv.window, 1
         return t
 
-    def _ref(self, obj):
-        self._keep.append(obj)
-        return obj
+    def ref(self, x):
+        """``byref`` of a ctypes structure, or of the descriptor of a view, kept alive with the executor (None: None)."""
+        if x is None:
+            return None
+        self._keep.append(self.tensor(x) if isinstance(x, TV) else x)
+        return C.byref(self._keep[-1])
 
-    def _dev(self, t: torch.Tensor) -> torch.Tensor:
-        """Packed parameter on the executor's device, kept alive with the executor."""
-        t = t.to(self.device).contiguous()
-        self._keep.append(t)
-        return t
+    def keep(self, t: torch.Tensor) -> int:
+        """Pointer of a packed parameter (or scratch) copied to the executor's device, kept alive with the executor."""
+        self._keep.append(t.to(self.device).contiguous())
+        return self._keep[-1].data_ptr()
 
-    def _bind(self, op):
-        lib = self.lib
-        if isinstance(op, ToNHWC):
-            bb, c, h, w = self.prog.inputs[op.src]
-            t = self._ref(self.tensor(op.out))
-            self.input_slots.setdefault(op.src, []).append((len(self.calls), 0))
-            self.calls.append(("ffcb_nchw_to_nhwc", lib.ffcb_nchw_to_nhwc, [None, bb, c, h, w, C.byref(t)]))
-        elif isinstance(op, ToNCHW):
-            t = self._ref(self.tensor(op.inp))
-            self.calls.append(("ffcb_nhwc_to_nchw", lib.ffcb_nhwc_to_nchw,
-                               [C.byref(t), self.outputs[op.dst].data_ptr()]))
-        elif isinstance(op, StemOp):
-            bb, c, h, w = self.prog.inputs[op.src]
-            t = self._ref(self.tensor(op.out))
-            wd, sd = self._dev(op.w), self._dev(op.shift)
-            self.input_slots.setdefault(op.src, []).append((len(self.calls), 0))
-            self.calls.append(("ffcb_stem_conv7", lib.ffcb_stem_conv7,
-                               [None, bb, c, h, w, wd.data_ptr(), sd.data_ptr(), wd.shape[1], C.byref(t)]))
-        elif isinstance(op, StemPackOp):
-            bb, c, h, w = self.prog.inputs[op.src]
-            t = self._ref(self.tensor(op.out))
-            self.input_slots.setdefault(op.src, []).append((len(self.calls), 0))
-            self.calls.append(("ffcb_stem_pack", lib.ffcb_stem_pack, [None, bb, c, h, w, C.byref(t)]))
-        elif isinstance(op, StemPackU8Op):
-            bb = self.prog.inputs[op.img][0]
-            t = self._ref(self.tensor(op.out))
-            self.input_slots.setdefault(op.img, []).append((len(self.calls), 0))
-            self.input_slots.setdefault(op.mask, []).append((len(self.calls), 1))
-            self.calls.append(("ffcb_stem_pack_u8", lib.ffcb_stem_pack_u8, [None, None, bb, op.h0, op.w0, C.byref(t)]))
-        elif isinstance(op, HeadGatherU8Op):
-            t = self._ref(self.tensor(op.q))
-            bd = self._dev(op.bias)
-            self.input_slots.setdefault(op.img, []).append((len(self.calls), 3))
-            self.input_slots.setdefault(op.mask, []).append((len(self.calls), 4))
-            self.calls.append(("ffcb_head_gather7_blend_u8", lib.ffcb_head_gather7_blend_u8,
-                               [C.byref(t), bd.data_ptr(), op.act, None, None, op.h0, op.w0,
-                                self.outputs[op.dst].data_ptr()]))
-        elif isinstance(op, HeadOp):
-            t = self._ref(self.tensor(op.inp))
-            wd, bd = self._dev(op.w), self._dev(op.bias)
-            self.calls.append(("ffcb_head_conv7", lib.ffcb_head_conv7,
-                               [C.byref(t), wd.data_ptr(), bd.data_ptr(), op.n_out, op.act,
-                                self.outputs[op.dst].data_ptr()]))
-        elif isinstance(op, HeadGatherOp):
-            t = self._ref(self.tensor(op.q))
-            bd = self._dev(op.bias)
-            self.calls.append(("ffcb_head_gather7", lib.ffcb_head_gather7,
-                               [C.byref(t), bd.data_ptr(), op.n_out, op.act, self.outputs[op.dst].data_ptr()]))
-        elif isinstance(op, ConvOp):
-            d = self._ref(L.ConvDesc())
-            pk = op.packed
-            d.inp[0] = self.tensor(op.ins[0])
-            if op.ins[1] is not None:
-                d.inp[1] = self.tensor(op.ins[1])
-            d.out = self.tensor(op.out)
-            if op.addend is not None:
-                d.addend = self.tensor(op.addend)
-            if self.prog.math == L.MATH_BF16X3:
-                wt = pk.split_weights()
-            else:
-                wt = pk.w_kn
-            d.weight = self._dev(wt).data_ptr()
-            if pk.shift is not None:
-                d.shift = self._dev(pk.shift).data_ptr()
-            d.n_out, d.stride, d.border, d.act = pk.n_out, pk.stride, pk.border, pk.act
-            d.nseg, d.math, d.addend_post = len(pk.segs), self.prog.math, int(op.addend_post)
-            for i, s in enumerate(pk.segs):
-                d.seg[i] = L.KSeg(s.src, s.dy, s.dx, s.c0, s.nch)
-            self.calls.append(("ffcb_conv:" + op.tag, lib.ffcb_conv, [C.byref(d)]))
-        elif isinstance(op, SplitOp):
-            self.split = len(self.calls)
-        elif isinstance(op, ReluBwdOp):
-            a, y, o = (self._ref(self.tensor(v)) for v in (op.dy, op.y, op.out))
-            self.calls.append(("ffcb_relu_bwd", lib.ffcb_relu_bwd, [C.byref(a), C.byref(y), C.byref(o)]))
-        elif isinstance(op, FoldOp):
-            g, o = self._ref(self.tensor(op.gpad)), self._ref(self.tensor(op.out))
-            adds = [(C.byref(self._ref(self.tensor(tv))), c0) for tv, c0 in op.addends] + [(None, 0)] * 2
-            self.calls.append(("ffcb_fold_reflect_border", lib.ffcb_fold_reflect_border,
-                               [C.byref(g), adds[0][0], adds[0][1], adds[1][0], adds[1][1], C.byref(o)]))
-        elif isinstance(op, AddOp):
-            a, bv, o = (self._ref(self.tensor(v)) for v in (op.a, op.b, op.out))
-            self.calls.append(("ffcb_add", lib.ffcb_add, [C.byref(a), C.byref(bv), C.byref(o)]))
-        elif isinstance(op, HeadBwdOp):
-            bb, n, h, w = self.prog.outputs[op.y]
-            m, o = self._ref(self.tensor(op.mask)), self._ref(self.tensor(op.out))
-            wd = self._dev(op.w)
-            dy = None
-            if op.dy in self.outputs:          # written by an earlier op of the program (RefineLossOp)
-                dy = self.outputs[op.dy].data_ptr()
-            else:
-                self.input_slots.setdefault(op.dy, []).append((len(self.calls), 1))
-            self.calls.append(("ffcb_head_bwd7", lib.ffcb_head_bwd7,
-                               [self.outputs[op.y].data_ptr(), dy, bb, n, h, w, wd.data_ptr(), op.act,
-                                C.byref(m), C.byref(o)]))
-        elif isinstance(op, RefineLossOp):
-            bb, n, hp, wp = self.prog.outputs[op.pred]
-            work = self._dev(torch.empty(op.ref_numel, dtype=torch.float32))
-            taps = self._dev(op.taps.float())
-            i = len(self.calls)
-            for name, ai in ((op.image, 1), (op.mask, 2), (op.ref, 9), (op.md, 10), (op.inv, 11)):
-                self.input_slots.setdefault(name, []).append((i, ai))
-            self.calls.append(("ffcb_refine_l1_grad", lib.ffcb_refine_l1_grad,
-                               [self.outputs[op.pred].data_ptr(), None, None, bb, n, hp, wp, op.h0, op.w0, None, None,
-                                None, taps.data_ptr(), work.data_ptr(), self.outputs[op.grad].data_ptr(),
-                                self.outputs[op.loss].data_ptr()]))
-        elif isinstance(op, BorderOp):
-            t = self._ref(self.tensor(op.view))
-            self.calls.append(("ffcb_fill_reflect_border", lib.ffcb_fill_reflect_border, [C.byref(t)]))
-        elif isinstance(op, RfftOp):
-            a, s = self._ref(self.tensor(op.inp)), self._ref(self.tensor(op.spec))
-            self.calls.append(("ffcb_rfft2", lib.ffcb_rfft2, [C.byref(a), C.byref(s), self.ws.data_ptr(), self.ws_bytes]))
-        elif isinstance(op, IrfftOp):
-            s, o = self._ref(self.tensor(op.spec)), self._ref(self.tensor(op.out))
-            r = C.byref(self._ref(self.tensor(op.residual))) if op.residual is not None else None
-            self.calls.append(("ffcb_irfft2", lib.ffcb_irfft2, [C.byref(s), r, C.byref(o), self.ws.data_ptr(), self.ws_bytes]))
-        else:
-            raise TypeError(op)
+    def bind_inputs(self, inputs: Dict[str, torch.Tensor]) -> None:
+        """Check each given input (on the executor's device type, declared dtype and shape, contiguous) and patch its
+        pointer into the calls that read it.  Inputs stay bound until rebound; the caller keeps them alive."""
+        for name, t in inputs.items():
+            shape, dt = tuple(self.prog.inputs[name]), self.prog.dtypes.get(name, torch.float32)
+            if not (t.device.type == self.device.type and t.dtype == dt and t.is_contiguous() and tuple(t.shape) == shape):
+                raise ValueError(f"input {name}: expected a contiguous {dt} {shape} on {self.device.type}, got "
+                                 f"{t.dtype} {tuple(t.shape)} on {t.device}")
+            for ci, ai in self.input_slots.get(name, ()):
+                self.calls[ci][2][ai] = t.data_ptr()
+            self._bound.add(name)
 
     def run(self, inputs: Dict[str, torch.Tensor], stream: Optional[int] = None,
             part: Optional[int] = None) -> Dict[str, torch.Tensor]:
-        """Issue every call on ``stream`` (default: torch's current stream).  Outputs are the
+        """Bind ``inputs`` and issue every call on ``stream`` (default: torch's current stream).  Outputs are the
         executor's own tensors (overwritten by the next run).  ``part``: 0 / 1 run only the forward / backward half
-        of a forward+backward program (inputs of the other half may be absent)."""
+        of a forward+backward program; inputs bound by an earlier run may be left out."""
         if torch.cuda.current_device() != self.dev_index:
             # the module lives on another GPU than the caller's current device (one process driving several GPUs):
             # kernels must be launched with that device current, as torch's own ops do through their device guards
             with torch.cuda.device(self.dev_index):
                 return self.run(inputs, stream, part)
+        if part not in self._parts:
+            raise ValueError(f"part={part}: not a forward+backward program")
+        lo, hi, needs = self._parts[part]
+        self.bind_inputs(inputs)
+        if not needs <= self._bound:
+            raise ValueError(f"inputs never bound: {sorted(needs - self._bound)}")
         if stream is None:
             stream = torch.cuda.current_stream(self.device).cuda_stream
-        if part is not None:
-            assert self.split is not None, "not a forward+backward program"
-            lo, hi = (0, self.split) if part == 0 else (self.split, len(self.calls))
-            for name, slots in self.input_slots.items():
-                if name in inputs:
-                    for ci, ai in slots:
-                        self.calls[ci][2][ai] = inputs[name].data_ptr()
-            for name, fn, args in self.calls[lo:hi]:
-                rc = fn(*args, stream)
-                if rc != 0:
-                    L.check(rc, name)
-            if part == 0:
-                self.generation += 1
-            return self.outputs
-        for name, slots in self.input_slots.items():
-            t = inputs[name]
-            dt = self.prog.dtypes.get(name, torch.float32)
-            assert t.is_cuda and t.dtype == dt and t.is_contiguous() and tuple(t.shape) == tuple(
-                self.prog.inputs[name]), f"input {name}: expected contiguous {dt} {self.prog.inputs[name]}"
-            for ci, ai in slots:
-                self.calls[ci][2][ai] = t.data_ptr()
-        first = self._launches is None
+        first = part is None and self._launches is None
         if first:
             self.lib.ffcb_reset_launch_count()
-        for name, fn, args in self.calls:
+        for name, fn, args in self.calls[lo:hi]:
             rc = fn(*args, stream)
             if rc != 0:
                 L.check(rc, name)
         if first:
             self._launches = int(self.lib.ffcb_launch_count())
+        if part == 0:
+            self.generation += 1
         return self.outputs
 
     @property
@@ -1686,65 +1704,43 @@ def get_executor(module, kind: str, tensors, math: Optional[int] = None,
     return ex
 
 
-class _BlockGradFn(torch.autograd.Function):
-    """FFCResnetBlock with native forward AND native input gradients (SURVEY.md row f3): what the reference's
-    refinement loop (evaluation/refinement.py:137-167) needs — it optimises the block inputs, the weights are frozen.
-    Forward runs the first half of a ``resnet_block_grad`` program (activations stay in the executor's buffers),
-    backward the second half.  One executor per (module, shape): a second forward before the backward of the first
-    would overwrite those activations, which raises instead of returning wrong gradients."""
+class _SplitProgramFn(torch.autograd.Function):
+    """Native forward AND native input gradients through a forward+backward program, weights frozen — what the
+    reference's refinement loop (evaluation/refinement.py:137-167) needs: ``resnet_block_grad`` for one FFCResnetBlock
+    (SURVEY.md row f3), ``generator_rear_grad`` for the whole rear (residual blocks, up-sampling tail, head).
+    Forward runs part 0 on inputs x0, x1 and returns the program outputs ``ys`` (plus x0 / x1 with ``residual``: the block
+    program leaves the identity add to the caller); backward runs part 1 on one gradient g<i> per output.  The forward's
+    activations stay in the executor's buffers, one executor per (module, shape): a second forward before the backward
+    of the first would overwrite them, which raises instead of returning wrong gradients."""
 
     @staticmethod
-    def forward(ctx, module, x_l, x_g):
-        ex = get_executor(module, "resnet_block_grad", (x_l, x_g))
-        xl, xg = x_l.detach().contiguous(), x_g.detach().contiguous()
-        outs = ex.run({"x0": xl, "x1": xg}, part=0)
-        ctx.ex, ctx.generation = ex, ex.generation
-        return xl + outs["y0"], xg + outs["y1"]
+    def forward(ctx, module, kind, ys, residual, what, x0, x1):
+        ex = get_executor(module, kind, (x0, x1))
+        xs = (x0.detach().contiguous(), x1.detach().contiguous())
+        outs = ex.run({"x0": xs[0], "x1": xs[1]}, part=0)
+        ctx.ex, ctx.generation, ctx.what = ex, ex.generation, what
+        res = tuple(x + outs[y] if residual else outs[y].clone() for y, x in zip(ys, xs))
+        return res if len(res) > 1 else res[0]
 
     @staticmethod
-    def backward(ctx, g_l, g_g):
+    def backward(ctx, *grads):
         ex = ctx.ex
         if ex.generation != ctx.generation:
-            raise RuntimeError("lama_b200: the same FFCResnetBlock ran forward again (same shape) before this backward; "
+            raise RuntimeError(f"lama_b200: {ctx.what} ran forward again (same shape) before this backward; "
                                "its saved activations were overwritten")
-        outs = ex.run({"g0": g_l.contiguous(), "g1": g_g.contiguous()}, part=1)
-        return None, outs["dx0"].clone(), outs["dx1"].clone()
+        outs = ex.run({f"g{i}": g.contiguous() for i, g in enumerate(grads)}, part=1)
+        return None, None, None, None, None, outs["dx0"].clone(), outs["dx1"].clone()
 
 
 def block_with_input_grad(module, x_l, x_g):
     """(out_l, out_g) of an FFCResnetBlock, differentiable w.r.t. x_l / x_g on the native path."""
-    return _BlockGradFn.apply(module, x_l, x_g)
-
-
-class _RearGradFn(torch.autograd.Function):
-    """``generator.model[first_block:]`` — residual blocks, up-sampling tail, head — with native forward AND native
-    input gradients: the whole rear of the refinement loop (evaluation/refinement.py:137-167) as ONE
-    ``generator_rear_grad`` program per (generator, shape).  Same contract as ``_BlockGradFn``: the forward part keeps
-    its activations in the executor's buffers, and a second forward before the backward raises."""
-
-    @staticmethod
-    def forward(ctx, gen, z1, z2):
-        ex = get_executor(gen, "generator_rear_grad", (z1, z2))
-        outs = ex.run({"x0": z1.detach().contiguous(), "x1": z2.detach().contiguous()}, part=0)
-        ctx.ex, ctx.generation = ex, ex.generation
-        return outs["y0"].clone()
-
-    @staticmethod
-    def backward(ctx, gy):
-        ex = ctx.ex
-        if ex.generation != ctx.generation:
-            raise RuntimeError("lama_b200: the generator's rear ran forward again (same shape) before this backward; "
-                               "its saved activations were overwritten")
-        gy = gy.contiguous()
-        assert gy.dtype == torch.float32 and tuple(gy.shape) == tuple(ex.prog.inputs["g0"])
-        outs = ex.run({"g0": gy}, part=1)
-        return None, outs["dx0"].clone(), outs["dx1"].clone()
+    return _SplitProgramFn.apply(module, "resnet_block_grad", ("y0", "y1"), True, "the same FFCResnetBlock", x_l, x_g)
 
 
 def generator_rear_with_input_grad(gen, z1, z2):
     """pred = ``gen.model[first_block:]((z1, z2))`` on the native path, differentiable w.r.t. z1 / z2 (the weights are
     frozen).  Callers check ``rear_grad_supported(gen, z1.shape, z2.shape)`` first."""
-    return _RearGradFn.apply(gen, z1, z2)
+    return _SplitProgramFn.apply(gen, "generator_rear_grad", ("y0",), False, "the generator's rear", z1, z2)
 
 
 def run_module(module, kind: str, tensors):

@@ -87,6 +87,26 @@ def ffc_resnet_block(x_l, x_g, sd, p, *, ratio_gout=0.75, enable_lfu=False):
     return x_l + y_l, x_g + y_g
 
 
+def generator_rear(z1, z2, sd, kw):
+    """``generator.model[first_block:]`` composed from the oracle: ffc_resnet_block per block, then ConvTranspose2d +
+    eval BN + ReLU per up stage, then reflect pad 3 + 7x7 conv + the head activation (ffc.py:345-363)."""
+    nd, nb = kw["n_downsampling"], kw["n_blocks"]
+    i = 2 + nd
+    z_l, z_g = z1, z2
+    for _ in range(nb):
+        z_l, z_g = ffc_resnet_block(z_l, z_g, sd, f"model.{i}.", ratio_gout=0.75); i += 1
+    h = torch.cat((z_l, z_g), dim=1); i += 1
+    for _ in range(nd):
+        h = F.conv_transpose2d(h, sd[f"model.{i}.weight"], sd[f"model.{i}.bias"], stride=2, padding=1,
+                               output_padding=1)
+        h = torch.relu(_bn(h, sd, f"model.{i + 1}.")); i += 3
+    h = F.conv2d(F.pad(h, (3, 3, 3, 3), mode="reflect"), sd[f"model.{i + 1}.weight"], sd[f"model.{i + 1}.bias"])
+    act = kw.get("add_out_act", True)
+    if act is True or act == "tanh":
+        return torch.tanh(h)
+    return torch.sigmoid(h) if act == "sigmoid" else h
+
+
 @torch.no_grad()
 def ffc_resnet_generator(x, sd, *, ngf=64, n_downsampling=3, n_blocks=9, init_conv_kwargs=None,
                          downsample_conv_kwargs=None, resnet_conv_kwargs=None, add_out_act=True,

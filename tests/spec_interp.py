@@ -4,7 +4,10 @@ product — BN folding, weight packing, K-segment lists, buffer wiring, residual
 sub-pixel phases — against the goldens on the GPU-less build box.  It is not a fallback: the
 product only executes programs through libffc_b200.so (lama_b200.engine.CudaExecutor).
 """
+from collections import ChainMap
+
 import torch
+import torch.nn.functional as F
 
 from lama_b200 import _lib as L
 from lama_b200 import engine as E
@@ -64,9 +67,7 @@ class SpecInterpreter:
         for n in range(n_out):
             g = q[:, :, :, n * 7:n * 7 + 7]                  # [B,H,W,7]
             ys.append(sum(g[:, :, xi[:, kx], kx] for kx in range(7)) + float(bias[n]))
-        y = torch.stack(ys, dim=1)
-        return {L.ACT_NONE: y, L.ACT_RELU: y.clamp_min(0), L.ACT_SIGMOID: torch.sigmoid(y),
-                L.ACT_TANH: torch.tanh(y)}[act]
+        return _ACT[act](torch.stack(ys, dim=1))
 
     @staticmethod
     def _two_rows(p, cin):
@@ -94,77 +95,182 @@ class SpecInterpreter:
         return out
 
     def step(self, op, inputs, out):
-        """Interpret one op: read its views from ``self.mem``, write its views there, and put external outputs
-        (ToNCHW, the heads) into ``out``.  ``inputs`` holds the program's external NCHW (or uint8) inputs."""
-        if isinstance(op, E.ToNHWC):
-            self.write(op.out, inputs[op.src].double().permute(0, 2, 3, 1))
-        elif isinstance(op, E.ToNCHW):
-            out[op.dst] = self.read(op.inp).permute(0, 3, 1, 2).contiguous()
-        elif isinstance(op, E.StemPackOp):
-            x = torch.nn.functional.pad(inputs[op.src].double(), (3, 3, 3, 3), mode="reflect")
-            x = torch.nn.functional.pad(x, (0, 2, 0, 0, 0, 8 - op.cin))          # W+6 -> W+8, Cin -> 8 (zeros)
-            self.write(op.out, self._two_rows(x.permute(0, 2, 3, 1), op.cin))
-        elif isinstance(op, E.StemPackU8Op):
-            x = self._u8_front(inputs[op.img], inputs[op.mask], op.out.buf.H - 6, op.out.buf.W - 8)
-            x = torch.nn.functional.pad(x.double(), (3, 3, 3, 3), mode="reflect")
-            x = torch.nn.functional.pad(x, (0, 2, 0, 0, 0, 4))
-            self.write(op.out, self._two_rows(x.permute(0, 2, 3, 1), 4))
-        elif isinstance(op, E.HeadGatherU8Op):
-            pred = self._gather(self.read(op.q), op.bias, 3, op.act).float()[:, :, :op.h0, :op.w0]
-            img = inputs[op.img].permute(0, 3, 1, 2).float() / 255
-            hole = (inputs[op.mask] > 0)[:, None]
-            res = torch.where(hole, pred, img)                      # mask*pred + (1-mask)*img, mask in {0,1}
-            out[op.dst] = (res * 255).clamp(0, 255).to(torch.uint8).permute(0, 2, 3, 1).contiguous()
-        elif isinstance(op, E.StemOp):
-            x = torch.nn.functional.pad(inputs[op.src].double(), (3, 3, 3, 3), mode="reflect")
-            cin = op.cin
-            w = op.w.double().to(x.device).reshape(7, 7, cin, -1).permute(3, 2, 0, 1)       # [N, Cin, 7, 7]
-            y = torch.nn.functional.conv2d(x, w) + op.shift.double().to(x.device)[None, :, None, None]
-            self.write(op.out, y.clamp_min(0).permute(0, 2, 3, 1))
-        elif isinstance(op, E.HeadOp):
-            x = self.read(op.inp).permute(0, 3, 1, 2)
-            x = torch.nn.functional.pad(x, (3, 3, 3, 3), mode="reflect")
-            w = op.w.double().to(x.device).reshape(op.n_out, 7, 7, -1).permute(0, 3, 1, 2)
-            y = torch.nn.functional.conv2d(x, w, op.bias.double().to(x.device))
-            y = {L.ACT_NONE: y, L.ACT_RELU: y.clamp_min(0), L.ACT_SIGMOID: torch.sigmoid(y),
-                 L.ACT_TANH: torch.tanh(y)}[op.act]
-            out[op.dst] = y
-        elif isinstance(op, E.HeadGatherOp):
-            out[op.dst] = self._gather(self.read(op.q), op.bias, op.n_out, op.act)
-        elif isinstance(op, E.ConvOp):
-            ins = [self.read(tv) if tv is not None else None for tv in op.ins]
-            assert all(not torch.isnan(t).any() for t in ins if t is not None), f"{op.tag}: reads unwritten data"
-            add = self.read(op.addend).clone() if op.addend is not None else None
-            y = apply_packed_reference(op.packed, ins, op.out.hw, addend=add, addend_post=op.addend_post)
-            self.write(op.out, y)
-        elif isinstance(op, E.BorderOp) or isinstance(op, E.SplitOp):
-            pass        # the interpreter's buffers have no physical ring (taps use index math)
-        elif isinstance(op, E.ReluBwdOp):
-            self.write(op.out, self.read(op.dy) * (self.read(op.y) > 0))
-        elif isinstance(op, E.FoldOp):
-            g = self.read(op.gpad)                                  # [B, H+2, W+2, C]
-            h, w = g.shape[1] - 2, g.shape[2] - 2
-            acc = torch.zeros(g.shape[0], h, w, g.shape[3], dtype=g.dtype)
-            for yp in range(h + 2):
-                y = abs(yp - 1); y = 2 * h - 2 - y if y >= h else y
-                for xp in range(w + 2):
-                    x = abs(xp - 1); x = 2 * w - 2 - x if x >= w else x
-                    acc[:, y, x] += g[:, yp, xp]
-            for tv, c0 in op.addends:
-                a = self.read(tv)
-                acc[..., c0:c0 + a.shape[-1]] += a
-            self.write(op.out, acc)
-        elif isinstance(op, E.RfftOp):
-            x = self.read(op.inp)                                            # [B,H,W,C]
-            f = torch.fft.rfftn(x, dim=(1, 2), norm="ortho")                 # [B,H,Wf,C]
-            self.write(op.spec, torch.view_as_real(f).reshape(*f.shape[:3], -1))   # channel 2c=Re, 2c+1=Im
-        elif isinstance(op, E.IrfftOp):
-            z = self.read(op.spec)
-            zc = torch.view_as_complex(z.reshape(*z.shape[:3], -1, 2).contiguous())
-            h, w = op.out.hw
-            y = torch.fft.irfftn(zc, s=(h, w), dim=(1, 2), norm="ortho")
-            if op.residual is not None:
-                y = y + self.read(op.residual)
-            self.write(op.out, y)
-        else:
-            raise TypeError(op)
+        """Interpret one op: read its views from ``self.mem``, write its views there.  Its external tensors resolve
+        from one namespace, as in the executor: the program's inputs (``inputs``) and the outputs written so far
+        (``out``); the outputs it writes go to ``out``."""
+        getattr(self, type(op).__name__)(op, ChainMap(out, inputs))
+
+    def ToNHWC(self, op, ext):
+        self.write(op.out, ext[op.src].double().permute(0, 2, 3, 1))
+
+    def ToNCHW(self, op, ext):
+        ext[op.dst] = self.read(op.inp).permute(0, 3, 1, 2).contiguous()
+
+    def StemPackOp(self, op, ext):
+        x = F.pad(ext[op.src].double(), (3, 3, 3, 3), mode="reflect")
+        x = F.pad(x, (0, 2, 0, 0, 0, 8 - op.cin))          # W+6 -> W+8, Cin -> 8 (zeros)
+        self.write(op.out, self._two_rows(x.permute(0, 2, 3, 1), op.cin))
+
+    def StemPackU8Op(self, op, ext):
+        x = self._u8_front(ext[op.img], ext[op.mask], op.out.buf.H - 6, op.out.buf.W - 8)
+        x = F.pad(x.double(), (3, 3, 3, 3), mode="reflect")
+        x = F.pad(x, (0, 2, 0, 0, 0, 4))
+        self.write(op.out, self._two_rows(x.permute(0, 2, 3, 1), 4))
+
+    def HeadGatherU8Op(self, op, ext):
+        pred = self._gather(self.read(op.q), op.bias, 3, op.act).float()[:, :, :op.h0, :op.w0]
+        img = ext[op.img].permute(0, 3, 1, 2).float() / 255
+        hole = (ext[op.mask] > 0)[:, None]
+        res = torch.where(hole, pred, img)                      # mask*pred + (1-mask)*img, mask in {0,1}
+        ext[op.dst] = (res * 255).clamp(0, 255).to(torch.uint8).permute(0, 2, 3, 1).contiguous()
+
+    def StemOp(self, op, ext):
+        x = F.pad(ext[op.src].double(), (3, 3, 3, 3), mode="reflect")
+        cin = op.cin
+        w = op.w.double().to(x.device).reshape(7, 7, cin, -1).permute(3, 2, 0, 1)       # [N, Cin, 7, 7]
+        y = F.conv2d(x, w) + op.shift.double().to(x.device)[None, :, None, None]
+        self.write(op.out, y.clamp_min(0).permute(0, 2, 3, 1))
+
+    def HeadOp(self, op, ext):
+        x = self.read(op.inp).permute(0, 3, 1, 2)
+        x = F.pad(x, (3, 3, 3, 3), mode="reflect")
+        w = op.w.double().to(x.device).reshape(op.n_out, 7, 7, -1).permute(0, 3, 1, 2)
+        ext[op.dst] = _ACT[op.act](F.conv2d(x, w, op.bias.double().to(x.device)))
+
+    def HeadGatherOp(self, op, ext):
+        ext[op.dst] = self._gather(self.read(op.q), op.bias, op.n_out, op.act)
+
+    def ConvOp(self, op, ext):
+        ins = [self.read(tv) if tv is not None else None for tv in op.ins]
+        assert all(not torch.isnan(t).any() for t in ins if t is not None), f"{op.tag}: reads unwritten data"
+        add = self.read(op.addend).clone() if op.addend is not None else None
+        y = apply_packed_reference(op.packed, ins, op.out.hw, addend=add, addend_post=op.addend_post)
+        self.write(op.out, y)
+
+    def BorderOp(self, op, ext):
+        pass        # the interpreter's buffers have no physical ring (taps use index math)
+
+    def SplitOp(self, op, ext):
+        pass
+
+    def ReluBwdOp(self, op, ext):
+        self.write(op.out, self.read(op.dy) * (self.read(op.y) > 0))
+
+    def FoldOp(self, op, ext):
+        g = self.read(op.gpad)                                  # [B, H+2, W+2, C]
+        h, w = g.shape[1] - 2, g.shape[2] - 2
+        acc = torch.zeros(g.shape[0], h, w, g.shape[3], dtype=g.dtype)
+        for yp in range(h + 2):
+            y = abs(yp - 1); y = 2 * h - 2 - y if y >= h else y
+            for xp in range(w + 2):
+                x = abs(xp - 1); x = 2 * w - 2 - x if x >= w else x
+                acc[:, y, x] += g[:, yp, xp]
+        for tv, c0 in op.addends:
+            a = self.read(tv)
+            acc[..., c0:c0 + a.shape[-1]] += a
+        self.write(op.out, acc)
+
+    def AddOp(self, op, ext):
+        self.write(op.out, self.read(op.a) + self.read(op.b))
+
+    def HeadBwdOp(self, op, ext):
+        y, dy = ext[op.y].double().cpu(), ext[op.dy].double().cpu()
+        d = {L.ACT_NONE: dy, L.ACT_SIGMOID: dy * y * (1 - y), L.ACT_TANH: dy * (1 - y * y)}[op.act]
+        w = op.w.double().cpu().reshape(op.n_out, 7, 7, -1).permute(0, 3, 1, 2)              # [N, C, 7, 7]
+        gp = F.conv_transpose2d(d, w)                                                     # [B, C, H+6, W+6]
+        h, wd = gp.shape[2] - 6, gp.shape[3] - 6
+        # Fold3: padded row / column p came from interior reflect(p - 3)
+        ry = (torch.arange(h + 6) - 3).abs(); ry = torch.where(ry >= h, 2 * h - 2 - ry, ry)
+        rx = (torch.arange(wd + 6) - 3).abs(); rx = torch.where(rx >= wd, 2 * wd - 2 - rx, rx)
+        g = torch.zeros(gp.shape[0], gp.shape[1], h, wd + 6, dtype=gp.dtype).index_add_(2, ry, gp)
+        g = torch.zeros(gp.shape[0], gp.shape[1], h, wd, dtype=gp.dtype).index_add_(3, rx, g)
+        m = self.read(op.mask)
+        self.write(op.out, g.permute(0, 2, 3, 1) * (m > 0))
+
+    def RefineLossOp(self, op, ext):
+        f = {k: ext[getattr(op, k)].double().cpu() for k in ("pred", "image", "mask", "ref", "md", "inv")}
+        ext[op.grad], ext[op.loss] = refine_loss_f64(f["pred"], f["image"], f["mask"], f["ref"], f["md"], f["inv"],
+                                                     op.h0, op.w0, op.taps)
+
+    def RfftOp(self, op, ext):
+        x = self.read(op.inp)                                            # [B,H,W,C]
+        f = torch.fft.rfftn(x, dim=(1, 2), norm="ortho")                 # [B,H,Wf,C]
+        self.write(op.spec, torch.view_as_real(f).reshape(*f.shape[:3], -1))   # channel 2c=Re, 2c+1=Im
+
+    def IrfftOp(self, op, ext):
+        z = self.read(op.spec)
+        zc = torch.view_as_complex(z.reshape(*z.shape[:3], -1, 2).contiguous())
+        h, w = op.out.hw
+        y = torch.fft.irfftn(zc, s=(h, w), dim=(1, 2), norm="ortho")
+        if op.residual is not None:
+            y = y + self.read(op.residual)
+        self.write(op.out, y)
+
+
+def storage_nbytes(b):
+    if b.tile:
+        return -(-(b.B * b.H * b.W) // 128) * 128 * b.C * 4
+    if b.cg:
+        return b.B * b.H * b.W * b.C * 4
+    return b.B * (b.H + 2 * b.pad) * (b.W + 2 * b.pad) * b.C * 4
+
+
+def check_liveness(prog):
+    """No two buffers of one storage slot are live at once (a forward write must survive to its backward read); returns
+    the pooled storage in bytes."""
+    slots = E.assign_storage_slots(prog)
+    first, last = {}, {}
+    for i, op in enumerate(prog.ops):
+        r, w = op.views()
+        for tv in r + w:
+            first.setdefault(tv.buf.name, i)
+            last[tv.buf.name] = i
+    by_slot = {}
+    for b in prog.bufs:
+        by_slot.setdefault(slots[b.name], []).append(b)
+    for members in by_slot.values():
+        assert len({E.storage_key(b) for b in members}) == 1
+        members = sorted(members, key=lambda b: first.get(b.name, -1))
+        for a, b in zip(members, members[1:]):
+            assert last[a.name] < first[b.name], (a.name, b.name)
+    return sum(storage_nbytes(m[0]) for m in by_slot.values())
+
+
+_ACT = {L.ACT_NONE: lambda y: y, L.ACT_RELU: lambda y: y.clamp_min(0), L.ACT_SIGMOID: torch.sigmoid,
+        L.ACT_TANH: torch.tanh}
+
+
+def _axis_matrix(n_in: int, taps) -> torch.Tensor:
+    """1-D operator of D along one axis, [n_in // 2, n_in]: bilinear (align_corners=False) rows of the 5-tap Gaussian
+    with reflect-101 padding (include/ffc_b200.h: ffcb_refine_l1_grad)."""
+    n_out = n_in // 2
+    scale = n_in / n_out
+    m = torch.zeros(n_out, n_in, dtype=torch.float64)
+    for d in range(n_out):
+        src = max(scale * (d + 0.5) - 0.5, 0.0)
+        i0 = int(src)
+        i1 = i0 + (1 if i0 < n_in - 1 else 0)
+        l1 = src - i0
+        for i, lam in ((i0, 1.0 - l1), (i1, l1)):
+            for a in range(5):
+                p = abs(i + a - 2)
+                p = 2 * n_in - 2 - p if p >= n_in else p
+                m[d, p] += lam * float(taps[a])
+    return m
+
+
+def refine_loss_f64(pred, image, mask, ref, md, inv, h0, w0, taps):
+    """(grad, loss (B,2)) of ffcb_refine_l1_grad in float64."""
+    inv = inv.double()
+    sel = (mask < 1e-8).double()
+    d = pred - image
+    grad = torch.sign(d) * sel * inv[:, 0, None, None, None]
+    my, mx = _axis_matrix(h0, taps), _axis_matrix(w0, taps)
+    e = torch.einsum("iy,bcyx,jx->bcij", my, pred[:, :, :h0, :w0], mx) - ref
+    seld = (md >= 1e-8).double()
+    r = torch.sign(e) * seld * inv[:, 1, None, None, None]
+    grad[:, :, :h0, :w0] += torch.einsum("iy,bcij,jx->bcyx", my, r, mx)
+    nan = torch.tensor(float("nan"), dtype=torch.float64)
+    l0 = torch.where(inv[:, 0] > 0, (d.abs() * sel).sum((1, 2, 3)) * inv[:, 0], nan)
+    l1 = torch.where(inv[:, 1] > 0, (e.abs() * seld).sum((1, 2, 3)) * inv[:, 1], nan)
+    return grad, torch.stack([l0, l1], 1)

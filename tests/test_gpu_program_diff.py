@@ -3,7 +3,8 @@
 1. Op by op (``diff_program``): one ``engine.Program`` is issued through ``CudaExecutor`` one C-ABI call at a time.
    Before each call the device buffers the op touches are decoded to float64 and loaded into ``SpecInterpreter``; after
    the call the interpreter runs that op alone and every view the op wrote is compared with what the kernel wrote.
-   Each op is judged on the device state it actually saw, so errors do not accumulate and a failure names one op.
+   Each op is judged on the device state it actually saw (its buffers, and the program outputs written so far), so
+   errors do not accumulate and a failure names one op.
    Before every reflect-border contraction the ring of each padded input must equal the reflection of its interior,
    bit for bit.
 2. Module level: FFCResnetBlock, FFC_BN_ACT, SpectralTransform and FourierUnit at 128-wide planes against the oracles,
@@ -123,17 +124,17 @@ def op_label(i, op) -> str:
     s = f"op {i} {type(op).__name__}"
     if isinstance(op, E.ConvOp):
         s += f" [{op.tag}]"
-    _, writes = E.op_views(op)
+    _, writes = op.views()
     return s + "".join(f" -> {tv.buf.name}" for tv in writes)
 
 
 def op_tol(op, math: int, out_fmt: int):
     """(limit on max-abs / max|ref|, compare against the split-bf16 rounding of the reference?)"""
-    if isinstance(op, (E.ConvOp, E.StemOp, E.HeadOp, E.HeadGatherOp)):           # contractions
+    if isinstance(op, (E.ConvOp, E.StemOp, E.HeadOp, E.HeadGatherOp, E.HeadBwdOp)):           # contractions
         return (2e-4 if math == L.MATH_BF16X3 else 2e-5), False
     if isinstance(op, (E.RfftOp, E.IrfftOp)):
         return (2e-5 if out_fmt == L.BF16X2 else 2e-6), False
-    return 1e-6, out_fmt == L.BF16X2           # layout, ring, ReLU backward, fold: exact up to the storage format
+    return 1e-6, out_fmt == L.BF16X2           # layout, ring, ReLU backward, fold, add, loss: exact up to the storage format
 
 
 def _rel(got, ref) -> float:
@@ -148,9 +149,7 @@ def diff_program(prog: E.Program, inputs, after_call=None):
     ex = E.CudaExecutor(prog, torch.device(DEV))
     assert len(ex.calls) == sum(not isinstance(op, E.SplitOp) for op in prog.ops)
     feed = {k: v.to(DEV).contiguous() for k, v in inputs.items()}
-    for name, slots in ex.input_slots.items():         # bind the input pointers as CudaExecutor.run does
-        for ci, ai in slots:
-            ex.calls[ci][2][ai] = feed[name].data_ptr()
+    ex.bind_inputs(feed)
     host_in = {k: v.cpu() for k, v in inputs.items()}
     dec = Decoder(ex)
     interp = SpecInterpreter(prog)
@@ -161,7 +160,7 @@ def diff_program(prog: E.Program, inputs, after_call=None):
     for i, op in enumerate(prog.ops):
         if isinstance(op, E.SplitOp):
             continue
-        reads, writes = E.op_views(op)
+        reads, writes = op.views()
         touched = {tv.buf.name: tv.buf for tv in reads + writes}
         for name, b in touched.items():
             interp.mem[name] = dec(b)
@@ -175,8 +174,9 @@ def diff_program(prog: E.Program, inputs, after_call=None):
         if after_call is not None:
             after_call(i, op, ex)
         torch.cuda.synchronize()
-        ref_ext = {}
-        interp.step(op, host_in, ref_ext)
+        out = {k: v.cpu() for k, v in ex.outputs.items()}     # the device's outputs as they stand before the call
+        before = dict(out)
+        interp.step(op, host_in, out)
         worst = None
         for tv in writes:
             ref = interp.read(tv)
@@ -188,9 +188,11 @@ def diff_program(prog: E.Program, inputs, after_call=None):
             err = _rel(got, split_bf16(ref) if rounded else ref)
             if not err <= tol:
                 worst = (i, op_label(i, op), err, tol)
-        for dst, ref in ref_ext.items():
+        for dst in prog.outputs:
+            if out[dst] is before[dst]:
+                continue                                # not written by this op
             tol, _ = op_tol(op, prog.math, L.F32)
-            err = _rel(ex.outputs[dst].cpu().double(), ref.double())
+            err = _rel(ex.outputs[dst].cpu().double(), out[dst].double())
             if not err <= tol:
                 worst = (i, op_label(i, op) + f" -> {dst}", err, tol)
         if worst is not None:
@@ -266,6 +268,31 @@ def test_generator_program_op_by_op(h, w, math):
     x = torch.cat([torch.rand(1, 3, h, w, generator=torch.Generator().manual_seed(5)),
                    (_randn(1, 1, h, w, seed=6) > 1.0).float()], dim=1)
     _diff(gen, "generator", ((1, 4, h, w),), {"x0": x}, math)
+
+
+@pytest.mark.parametrize("math", ["fp32", "bf16x3"])
+@pytest.mark.parametrize("kind", ["generator_rear_grad", "generator_refine:61x59"])
+def test_refinement_programs_op_by_op(kind, math):
+    """The refinement programs of the small generator: the rear's forward with the kept Y2 added back (ffcb_add), the
+    head adjoint, the transposed up-sampling convolutions and the block backwards; in the step program also the loss
+    gradient, judged at the 1e-6 of its kernel test, whose output the head adjoint reads."""
+    gen = seeded_parameters_(M.FFCResNetGenerator(**small_lama_kwargs(ngf=8, n_blocks=2)).eval(), 5, gain=1.0)
+    b, h, w = 2, 8, 8
+    sl, sg, img = (b, 16, h, w), (b, 48, h, w), (b, 3, 8 * h, 8 * w)
+    feed = {"x0": _randn(*sl, seed=1), "x1": _randn(*sg, seed=2)}
+    if kind == "generator_rear_grad":
+        feed["g0"] = _randn(*img, seed=3)
+    else:
+        h0, w0 = 61, 59
+        g = torch.Generator().manual_seed(4)
+        mask = torch.zeros(b, 1, *img[2:])
+        mask[0, :, 10:40, 12:44] = 1
+        mask[1, :, 30:60, 5:25] = 1
+        md = (torch.rand(b, 1, h0 // 2, w0 // 2, generator=g) > 0.5).float()
+        n = torch.stack([3 * (mask < 1e-8).sum((1, 2, 3)), 3 * (md >= 1e-8).sum((1, 2, 3))], 1)
+        feed.update(image=torch.rand(*img, generator=g), mask=mask, md=md, inv=1.0 / n,
+                    ref=torch.rand(b, 3, h0 // 2, w0 // 2, generator=g))
+    _diff(gen, kind, (sl, sg), feed, math)
 
 
 def test_harness_flags_a_corrupted_op():

@@ -128,7 +128,7 @@ def test_graph_replay_equals_eager_steps(math_mode):
     for lane in graphed._lanes.values():
         ex = lane.ex
         alloc = (ex.storage_bytes + ex.ws.numel() + sum(t.numel() * t.element_size() for t in ex.outputs.values())
-                 + sum(E.op_scratch_bytes(op) for op in ex.prog.ops))
+                 + sum(op.scratch_bytes() for op in ex.prog.ops))
         assert alloc == E.program_storage_bytes(ex.prog)
 
 

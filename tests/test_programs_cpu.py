@@ -368,7 +368,7 @@ def test_storage_slots_never_alias_live_buffers(monkeypatch):
     slots = E.assign_storage_slots(prog)
     first, last = {}, {}
     for i, op in enumerate(prog.ops):
-        r, w = E.op_views(op)
+        r, w = op.views()
         for tv in r + w:
             first.setdefault(tv.buf.name, i)
             last[tv.buf.name] = i

@@ -15,60 +15,10 @@ from lama_b200 import modules as M
 from lama_b200 import predict as PR
 from lama_b200 import refine as R
 from lama_b200.testing import BIG_LAMA_KWARGS, seeded_parameters_, small_lama_kwargs
-from test_refine_rear_cpu import RearSpecInterpreter, _check_liveness, _nbytes, rear_oracle
+from oracle import ffc_torch_cpu as otc
+from spec_interp import SpecInterpreter, check_liveness, refine_loss_f64, storage_nbytes
 
 GOLDEN_REAR_OPS = os.path.join(os.path.dirname(__file__), "golden", "rear_grad_program_ops.json")
-
-
-# ------------------------------------------------------------------------------------------- float64 restatement
-def _axis_matrix(n_in: int, taps) -> torch.Tensor:
-    """1-D operator of D along one axis, [n_in // 2, n_in]: bilinear (align_corners=False) rows of the 5-tap Gaussian
-    with reflect-101 padding (include/ffc_b200.h: ffcb_refine_l1_grad)."""
-    n_out = n_in // 2
-    scale = n_in / n_out
-    m = torch.zeros(n_out, n_in, dtype=torch.float64)
-    for d in range(n_out):
-        src = max(scale * (d + 0.5) - 0.5, 0.0)
-        i0 = int(src)
-        i1 = i0 + (1 if i0 < n_in - 1 else 0)
-        l1 = src - i0
-        for i, lam in ((i0, 1.0 - l1), (i1, l1)):
-            for a in range(5):
-                p = abs(i + a - 2)
-                p = 2 * n_in - 2 - p if p >= n_in else p
-                m[d, p] += lam * float(taps[a])
-    return m
-
-
-def refine_loss_f64(pred, image, mask, ref, md, inv, h0, w0, taps):
-    """(grad, loss (B,2)) of ffcb_refine_l1_grad in float64."""
-    inv = inv.double()
-    sel = (mask < 1e-8).double()
-    d = pred - image
-    grad = torch.sign(d) * sel * inv[:, 0, None, None, None]
-    my, mx = _axis_matrix(h0, taps), _axis_matrix(w0, taps)
-    e = torch.einsum("iy,bcyx,jx->bcij", my, pred[:, :, :h0, :w0], mx) - ref
-    seld = (md >= 1e-8).double()
-    r = torch.sign(e) * seld * inv[:, 1, None, None, None]
-    grad[:, :, :h0, :w0] += torch.einsum("iy,bcij,jx->bcyx", my, r, mx)
-    nan = torch.tensor(float("nan"), dtype=torch.float64)
-    l0 = torch.where(inv[:, 0] > 0, (d.abs() * sel).sum((1, 2, 3)) * inv[:, 0], nan)
-    l1 = torch.where(inv[:, 1] > 0, (e.abs() * seld).sum((1, 2, 3)) * inv[:, 1], nan)
-    return grad, torch.stack([l0, l1], 1)
-
-
-class RefineSpecInterpreter(RearSpecInterpreter):
-    """RearSpecInterpreter plus the refinement-loss op; the head adjoint reads the gradient that op wrote."""
-
-    def step(self, op, inputs, out):
-        if isinstance(op, E.RefineLossOp):
-            f = {k: inputs[getattr(op, k)].double() for k in ("image", "mask", "ref", "md", "inv")}
-            out[op.grad], out[op.loss] = refine_loss_f64(out[op.pred].double(), f["image"], f["mask"], f["ref"],
-                                                         f["md"], f["inv"], op.h0, op.w0, op.taps)
-        elif isinstance(op, E.HeadBwdOp) and op.dy in out:
-            super().step(op, {**inputs, op.dy: out[op.dy]}, out)
-        else:
-            super().step(op, inputs, out)
 
 
 @pytest.fixture
@@ -160,10 +110,10 @@ def test_refine_program_matches_autograd(math, f32_taps):
     z1, z2 = torch.randn(sl, generator=g), torch.randn(sg, generator=g)
     _, image, mask, ref, md = loss_case(b, 8 * h, 8 * w, h0, w0, seed=2, empty=(1,), equal=False)
     inv = counts(mask, md)
-    out = RefineSpecInterpreter(prog).run(dict(x0=z1, x1=z2, image=image, mask=mask, ref=ref, md=md, inv=inv))
+    out = SpecInterpreter(prog).run(dict(x0=z1, x1=z2, image=image, mask=mask, ref=ref, md=md, inv=inv))
     sd = {k: v.detach().double() for k, v in gen.state_dict().items()}
     a, c = z1.double().requires_grad_(True), z2.double().requires_grad_(True)
-    pred = rear_oracle(a, c, sd, kw)
+    pred = otc.generator_rear(a, c, sd, kw)
     want_g, want_loss = autograd_loss(pred.detach(), image, mask, ref, md, h0, w0)
     pred.backward(want_g)
     for got, want in ((out["y0"], pred.detach()), (out["dx0"], a.grad), (out["dx1"], c.grad), (out["dy0"], want_g)):
@@ -176,7 +126,7 @@ def op_signature(prog):
     """Op kinds, tags and every view's buffer (name, shape, format, ring, layout) and slice, in program order."""
     sig = []
     for op in prog.ops:
-        reads, writes = E.op_views(op)
+        reads, writes = op.views()
         views = [[tv.buf.name, tv.buf.B, tv.buf.H, tv.buf.W, tv.buf.C, tv.buf.pad, tv.buf.fmt, tv.buf.reflect_border,
                   tv.buf.cg, tv.buf.tile, tv.c0, tv.channels, list(tv.phase) if tv.phase else None, tv.window, tv.b0,
                   tv.batch, list(tv.win) if tv.win else None, tv.bcast] for tv in reads + writes]
@@ -241,7 +191,7 @@ def test_program_storage_bytes():
             progs[b] = E.build_module_program(gen, "generator_refine:45x77", ((b, 16, 6, 10), (b, 48, 6, 10)),
                                               L.MATH_BF16X3)
     p = progs[3]
-    want = (_check_liveness(p) + sum(4 * int(np.prod(s)) for s in p.outputs.values()) + p.fft_workspace_bytes()
+    want = (check_liveness(p) + sum(4 * int(np.prod(s)) for s in p.outputs.values()) + p.fft_workspace_bytes()
             + 4 * 3 * 3 * 22 * 38)
     assert E.program_storage_bytes(p) == want
     one, three = E.program_storage_bytes(progs[1]), E.program_storage_bytes(progs[3])
@@ -251,7 +201,7 @@ def test_program_storage_bytes():
         bp = E.build_module_program(big, "generator_refine:1344x1344", ((1, 128, 168, 168), (1, 384, 168, 168)),
                                     L.MATH_BF16X3)
     print(f"big-lama step program at 1344x1344: {E.program_storage_bytes(bp) / 1e9:.2f} GB")
-    assert E.program_storage_bytes(bp) > _nbytes(bp.bufs[0])
+    assert E.program_storage_bytes(bp) > storage_nbytes(bp.bufs[0])
 
 
 def test_plan_batches():
