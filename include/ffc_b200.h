@@ -187,8 +187,11 @@ int ffcb_head_conv7(const ffcb_tensor* in, const float* w, const float* bias, in
  * The inverse transforms along H first (all W/2+1 columns, complex) and then C2R along W,
  * ignoring Im of the k_w=0 and (even W) k_w=W/2 bins — exactly what torch/cuFFT/MKL do for the
  * non-Hermitian post-ReLU spectrum (SURVEY.md Appendix A).
- * Power-of-two H, W in [4, 256] take the shared-memory Stockham kernels; any other size takes
- * a direct-DFT kernel (exact same results, O(n^2)).
+ * H and W may be any length from 1 to 1024 (W >= 2); longer axes return FFCB_EINVAL.  Most 64x64
+ * planes take a fused whole-plane kernel; every other plane takes a row and a column kernel with
+ * the transform in shared memory: power-of-two lengths 4..256 a compile-time Stockham plan,
+ * every other length a runtime mixed-radix Stockham plan (a direct DFT for primes), with 32
+ * channels per CTA up to 447 points and 8 channels per CTA for 448..1024.
  * ws: caller workspace of ffcb_fft2_workspace_bytes(B,H,W,C) bytes (row-pass intermediate).
  */
 size_t ffcb_fft2_workspace_bytes(int B, int H, int W, int C);

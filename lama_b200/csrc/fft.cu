@@ -11,8 +11,15 @@
 // sizes of the path); rows are transformed two at a time ("two-for-one": z = row_a + i*row_b).
 //
 // Sizes: power-of-two lengths 4..256 run a mixed-radix (8/4) Stockham autosort (ping-pong buffers);
-// every other length runs a direct DFT (same kernels, O(n^2)) so odd / non-power-of-two planes
-// (bin/predict.py pads images to multiples of 8 only -> e.g. 125x188 bottlenecks) stay native.
+// every other length runs the runtime mixed-radix Stockham (a direct DFT for primes), so odd /
+// non-power-of-two planes (bin/predict.py pads images to multiples of 8 only -> e.g. 125x188
+// bottlenecks) stay native.
+//
+// Channels per CTA (template L): 32, or 8 for lengths 448..1024, whose 32-channel ping-pong buffers
+// (8 * (n + 64 n) bytes) exceed the 227 KB of shared memory a CTA may hold; the 8-channel CTA needs
+// 8 * (n + 16 n) bytes (139 KB at 1024).  With L = 8 a warp covers 8 channels x 4 workers, so every
+// global access still moves whole 32-byte sectors.  These lengths are the bottlenecks of 4K and
+// larger photos (3840x2160 -> 480x270, 4000x3000 -> 500x375, 4096^2 -> 512^2).
 #include <math.h>
 #include <stdlib.h>
 
@@ -22,40 +29,42 @@
 namespace ffcb {
 namespace {
 
-constexpr int kLanes = 32;
+constexpr int kLanes = 32;        // channels per CTA of every length whose buffers fit
+constexpr int kNarrowLanes = 8;   // channels per CTA of lengths 448..1024
+constexpr int kMaxLen = 1024;     // longest axis (make_rt_plan factors every length up to 1024)
 using namespace fftc;
 
 // Complex FFT of length N (compile-time power of two, or runtime n when N == 0) for this lane.
 // `a` holds the input (already synchronised), `b` is scratch of the same size; returns the
 // buffer holding the result.  Ends with a barrier.
-template <int N, bool INV>
+template <int N, int L, bool INV>
 __device__ __forceinline__ float2* fft_dispatch(float2* a, float2* b, const float2* tw, int n, int lane, int worker,
                                                 int nworkers, const RtPlan& rp) {
   if constexpr (N == 0) {
     if (rp.np < 0) {                       // direct DFT
-      dft_pass<INV, kLanes>(a, b, tw, n, lane, worker, nworkers);
+      dft_pass<INV, L>(a, b, tw, n, lane, worker, nworkers);
       __syncthreads();
       return b;
     }
     int ns = 1;                            // runtime mixed-radix Stockham (row f2)
     for (int p = 0; p < rp.np; ++p) {
       const int R = rp.radix[p];
-      generic_pass<INV, kLanes>(a, b, tw, n, R, ns, lane, worker, nworkers);
+      generic_pass<INV, L>(a, b, tw, n, R, ns, lane, worker, nworkers);
       __syncthreads();
       ns *= R;
       float2* t = a; a = b; b = t;
     }
     return a;
   } else {
-    stockham_pass<N, 0, INV, kLanes>(a, b, tw, lane, worker, nworkers);
+    stockham_pass<N, 0, INV, L>(a, b, tw, lane, worker, nworkers);
     __syncthreads();
     if constexpr (Plan<N>::P == 1) return b;
     else {
-      stockham_pass<N, 1, INV, kLanes>(b, a, tw, lane, worker, nworkers);
+      stockham_pass<N, 1, INV, L>(b, a, tw, lane, worker, nworkers);
       __syncthreads();
       if constexpr (Plan<N>::P == 2) return a;
       else {
-        stockham_pass<N, 2, INV, kLanes>(a, b, tw, lane, worker, nworkers);
+        stockham_pass<N, 2, INV, L>(a, b, tw, lane, worker, nworkers);
         __syncthreads();
         return b;
       }
@@ -73,24 +82,24 @@ __device__ __forceinline__ void make_twiddles(float2* tw, int n) {
   }
 }
 
-// Shared-memory carve-up: [twiddles n][group g: ping n*32 | pong n*32]
-template <int N>
+// Shared-memory carve-up: [twiddles n][group g: ping n*L | pong n*L]
+template <int N, int L>
 __device__ __forceinline__ void carve(float2* smem, int n, int group, float2*& tw, float2*& data, float2*& tmp) {
   tw = smem;
-  data = smem + n + (size_t)group * 2 * n * kLanes;
-  tmp = data + n * kLanes;
+  data = smem + n + (size_t)group * 2 * n * L;
+  tmp = data + n * L;
 }
 
 // ---------------------------------------------------------------------------------------------
-// Row pass, forward.  grid.x = ceil(B*ceil(H/2) / G), grid.y = ceil(C/32).
+// Row pass, forward.  grid.x = ceil(B*ceil(H/2) / G), grid.y = ceil(C/L).
 // in (B,H,W,C) real  ->  ws[b][y][k][c] complex, k = 0..W/2   (unscaled)
-template <int N>
+template <int N, int L>
 __global__ void __launch_bounds__(1024) rfft_rows_kernel(View in, float2* __restrict__ ws, int n, RtPlan rp) {
   extern __shared__ float2 smem_f2[];
   const int W = (N > 0) ? N : n;
   const int lane = threadIdx.x, worker = threadIdx.y, nworkers = blockDim.y, group = threadIdx.z;
   float2 *tw, *data, *tmp;
-  carve<N>(smem_f2, W, group, tw, data, tmp);
+  carve<N, L>(smem_f2, W, group, tw, data, tmp);
   make_twiddles(tw, W);
 
   const int hp = (in.H + 1) / 2;
@@ -98,7 +107,7 @@ __global__ void __launch_bounds__(1024) rfft_rows_kernel(View in, float2* __rest
   const bool live = pair < in.B * hp;
   const int b = live ? pair / hp : 0;
   const int y0 = live ? (pair % hp) * 2 : 0;
-  const int c = blockIdx.y * kLanes + lane;
+  const int c = blockIdx.y * L + lane;
   const bool cok = live && c < in.C;
   const bool row1 = (y0 + 1) < in.H;
 
@@ -108,16 +117,16 @@ __global__ void __launch_bounds__(1024) rfft_rows_kernel(View in, float2* __rest
       z.x = load1(in, pix_off(in, b, y0, x) + c);
       if (row1) z.y = load1(in, pix_off(in, b, y0 + 1, x) + c);
     }
-    data[x * kLanes + lane] = z;
+    data[x * L + lane] = z;
   }
   __syncthreads();
-  const float2* res = fft_dispatch<N, false>(data, tmp, tw, W, lane, worker, nworkers, rp);
+  const float2* res = fft_dispatch<N, L, false>(data, tmp, tw, W, lane, worker, nworkers, rp);
 
   const int wf = W / 2 + 1;
   if (cok) {
     for (int k = worker; k < wf; k += nworkers) {
       float2 a, bb;
-      r2c_pair_post<kLanes>(res, W, k, lane, a, bb);
+      r2c_pair_post<L>(res, W, k, lane, a, bb);
       const size_t o = (((size_t)b * in.H + y0) * wf + k) * in.C + c;
       ws[o] = a;
       if (row1) ws[o + (size_t)wf * in.C] = bb;
@@ -125,16 +134,16 @@ __global__ void __launch_bounds__(1024) rfft_rows_kernel(View in, float2* __rest
   }
 }
 
-// Column pass, forward.  grid.x = ceil(B*Wf / G), grid.y = ceil(C/32).
+// Column pass, forward.  grid.x = ceil(B*Wf / G), grid.y = ceil(C/L).
 // ws[b][y][k][c] complex -> spec (B,H,Wf,2C): channel 2c = Re, 2c+1 = Im, scaled by `scale`.
-template <int N>
+template <int N, int L>
 __global__ void __launch_bounds__(1024) fft_cols_fwd_kernel(const float2* __restrict__ ws, View spec, int n,
                                                             int C, float scale, RtPlan rp) {
   extern __shared__ float2 smem_f2[];
   const int H = (N > 0) ? N : n;
   const int lane = threadIdx.x, worker = threadIdx.y, nworkers = blockDim.y, group = threadIdx.z;
   float2 *tw, *data, *tmp;
-  carve<N>(smem_f2, H, group, tw, data, tmp);
+  carve<N, L>(smem_f2, H, group, tw, data, tmp);
   make_twiddles(tw, H);
 
   const int wf = spec.W;
@@ -142,20 +151,20 @@ __global__ void __launch_bounds__(1024) fft_cols_fwd_kernel(const float2* __rest
   const bool live = col < spec.B * wf;
   const int b = live ? col / wf : 0;
   const int k = live ? col % wf : 0;
-  const int c = blockIdx.y * kLanes + lane;
+  const int c = blockIdx.y * L + lane;
   const bool cok = live && c < C;
 
   for (int y = worker; y < H; y += nworkers) {
     float2 z = make_float2(0.f, 0.f);
     if (cok) z = ws[(((size_t)b * H + y) * wf + k) * C + c];
-    data[y * kLanes + lane] = z;
+    data[y * L + lane] = z;
   }
   __syncthreads();
-  const float2* res = fft_dispatch<N, false>(data, tmp, tw, H, lane, worker, nworkers, rp);
+  const float2* res = fft_dispatch<N, L, false>(data, tmp, tw, H, lane, worker, nworkers, rp);
 
   if (cok) {
     for (int y = worker; y < H; y += nworkers) {
-      const float2 z = res[y * kLanes + lane];
+      const float2 z = res[y * L + lane];
       const long long o = pix_off(spec, b, y, k) + 2 * c;
       if (spec.fmt == FFCB_F32) {
         *reinterpret_cast<float2*>(reinterpret_cast<float*>(spec.ptr) + o) = make_float2(z.x * scale, z.y * scale);
@@ -173,13 +182,13 @@ __global__ void __launch_bounds__(1024) fft_cols_fwd_kernel(const float2* __rest
 }
 
 // Column pass, inverse: spec (B,H,Wf,2C) -> ws[b][y][k][c] complex (unscaled inverse along H).
-template <int N>
+template <int N, int L>
 __global__ void __launch_bounds__(N > 0 && N <= 64 ? 256 : 1024, N > 0 && N <= 64 ? 6 : 1) fft_cols_inv_kernel(View spec, float2* __restrict__ ws, int n, int C, RtPlan rp) {
   extern __shared__ float2 smem_f2[];
   const int H = (N > 0) ? N : n;
   const int lane = threadIdx.x, worker = threadIdx.y, nworkers = blockDim.y, group = threadIdx.z;
   float2 *tw, *data, *tmp;
-  carve<N>(smem_f2, H, group, tw, data, tmp);
+  carve<N, L>(smem_f2, H, group, tw, data, tmp);
   make_twiddles(tw, H);
 
   const int wf = spec.W;
@@ -187,7 +196,7 @@ __global__ void __launch_bounds__(N > 0 && N <= 64 ? 256 : 1024, N > 0 && N <= 6
   const bool live = col < spec.B * wf;
   const int b = live ? col / wf : 0;
   const int k = live ? col % wf : 0;
-  const int c = blockIdx.y * kLanes + lane;
+  const int c = blockIdx.y * L + lane;
   const bool cok = live && c < C;
 
   for (int y = worker; y < H; y += nworkers) {
@@ -201,27 +210,27 @@ __global__ void __launch_bounds__(N > 0 && N <= 64 ? 256 : 1024, N > 0 && N <= 6
         z.y = load1(spec, o + 1);
       }
     }
-    data[y * kLanes + lane] = z;
+    data[y * L + lane] = z;
   }
   __syncthreads();
-  const float2* res = fft_dispatch<N, true>(data, tmp, tw, H, lane, worker, nworkers, rp);
+  const float2* res = fft_dispatch<N, L, true>(data, tmp, tw, H, lane, worker, nworkers, rp);
 
   if (cok) {
     for (int y = worker; y < H; y += nworkers)
-      ws[(((size_t)b * H + y) * wf + k) * C + c] = res[y * kLanes + lane];
+      ws[(((size_t)b * H + y) * wf + k) * C + c] = res[y * L + lane];
   }
 }
 
 // Row pass, inverse (C2R, two rows at a time): ws[b][y][k][c] -> out (B,H,W,C) real,
 // out = residual + scale * c2r(ws).  Im of bins 0 and (even W) W/2 is ignored.
-template <int N>
+template <int N, int L>
 __global__ void __launch_bounds__(N > 0 && N <= 64 ? 256 : 1024, N > 0 && N <= 64 ? 6 : 1) irfft_rows_kernel(const float2* __restrict__ ws, View res, View out, int n,
                                                           float scale, RtPlan rp) {
   extern __shared__ float2 smem_f2[];
   const int W = (N > 0) ? N : n;
   const int lane = threadIdx.x, worker = threadIdx.y, nworkers = blockDim.y, group = threadIdx.z;
   float2 *tw, *data, *tmp;
-  carve<N>(smem_f2, W, group, tw, data, tmp);
+  carve<N, L>(smem_f2, W, group, tw, data, tmp);
   make_twiddles(tw, W);
 
   const int hp = (out.H + 1) / 2;
@@ -229,7 +238,7 @@ __global__ void __launch_bounds__(N > 0 && N <= 64 ? 256 : 1024, N > 0 && N <= 6
   const bool live = pair < out.B * hp;
   const int b = live ? pair / hp : 0;
   const int y0 = live ? (pair % hp) * 2 : 0;
-  const int c = blockIdx.y * kLanes + lane;
+  const int c = blockIdx.y * L + lane;
   const bool cok = live && c < out.C;
   const bool row1 = (y0 + 1) < out.H;
   const int wf = W / 2 + 1;
@@ -241,10 +250,10 @@ __global__ void __launch_bounds__(N > 0 && N <= 64 ? 256 : 1024, N > 0 && N <= 6
       x1 = ws[o];
       if (row1) x2 = ws[o + (size_t)wf * out.C];
     }
-    c2r_pair_pre<kLanes>(data, W, k, lane, x1, x2);
+    c2r_pair_pre<L>(data, W, k, lane, x1, x2);
   }
   __syncthreads();
-  const float2* fin = fft_dispatch<N, true>(data, tmp, tw, W, lane, worker, nworkers, rp);
+  const float2* fin = fft_dispatch<N, L, true>(data, tmp, tw, W, lane, worker, nworkers, rp);
 
   if (cok) {
     if (N > 0) {
@@ -262,14 +271,14 @@ __global__ void __launch_bounds__(N > 0 && N <= 64 ? 256 : 1024, N > 0 && N <= 6
       for (int i = 0; i < 8; ++i) {
         const int x = worker + i * nworkers;
         if (x < W) {
-          const float2 z = fin[x * kLanes + lane];
+          const float2 z = fin[x * L + lane];
           store1(out, o0 + x * out.sx, fmaf(z.x, scale, ra[i]));
           if (row1) store1(out, o0 + out.sy + x * out.sx, fmaf(z.y, scale, rb[i]));
         }
       }
     } else {
       for (int x = worker; x < W; x += nworkers) {
-        const float2 z = fin[x * kLanes + lane];
+        const float2 z = fin[x * L + lane];
         float r0 = z.x * scale, r1 = z.y * scale;
         if (res.ptr != nullptr) {
           r0 += load1(res, pix_off(res, b, y0, x) + c);
@@ -284,9 +293,10 @@ __global__ void __launch_bounds__(N > 0 && N <= 64 ? 256 : 1024, N > 0 && N <= 6
 
 // ---------------------------------------------------------------------------------------------
 struct LaunchPlan {
-  int N;       // template length (0 = direct DFT)
+  int N;       // template length (0 = runtime length)
   int n;       // runtime length
-  dim3 block;  // (32, workers, groups)
+  int lanes;   // channels per CTA: kLanes, or kNarrowLanes (N == 0 only)
+  dim3 block;  // (lanes, workers, groups)
   size_t smem;
   RtPlan rp;   // N == 0: runtime radix plan (np < 0: direct DFT)
 };
@@ -300,9 +310,16 @@ bool mixed_radix_enabled() {
 
 bool is_pow2(int v) { return v > 0 && (v & (v - 1)) == 0; }
 
+constexpr size_t kMaxSmem = 227 * 1024;
+
+size_t two_pass_smem(int n, int lanes, int groups) {
+  return sizeof(float2) * ((size_t)n + (size_t)groups * 2 * n * lanes);
+}
+
 LaunchPlan make_plan(int n) {
   LaunchPlan p;
   p.n = n;
+  p.lanes = kLanes;
   p.rp.np = -1;
   for (int i = 0; i < kMaxRtPasses; ++i) p.rp.radix[i] = 1;
   if (is_pow2(n) && n >= 4 && n <= 256) {
@@ -310,8 +327,8 @@ LaunchPlan make_plan(int n) {
     const int workers = fftc::workers_for(n);
     const int groups = workers >= 8 ? 1 : 8 / workers;
     p.block = dim3(kLanes, workers, groups);
-    p.smem = sizeof(float2) * ((size_t)n + (size_t)groups * 2 * n * kLanes);
-  } else {
+    p.smem = two_pass_smem(n, kLanes, groups);
+  } else if (two_pass_smem(n, kLanes, 1) <= kMaxSmem) {
     p.N = 0;
     int workers = n >= 8 ? 8 : (n >= 4 ? 4 : 1);
     if (mixed_radix_enabled()) {
@@ -321,12 +338,19 @@ LaunchPlan make_plan(int n) {
     }
     const int groups = n <= 32 ? (8 / workers > 0 ? 8 / workers : 1) : 1;
     p.block = dim3(kLanes, workers, groups);
-    p.smem = sizeof(float2) * ((size_t)n + (size_t)groups * 2 * n * kLanes);
+    p.smem = two_pass_smem(n, kLanes, groups);
+  } else {
+    // 448..1024 (longer lengths are rejected by check_fft_shapes): 8 channels per CTA, ~8 outputs per worker and
+    // pass, up to a full 1024-thread CTA
+    p.N = 0;
+    p.lanes = kNarrowLanes;
+    if (mixed_radix_enabled()) p.rp = make_rt_plan(n);
+    const int workers = (n + 7) / 8 < 1024 / kNarrowLanes ? (n + 7) / 8 : 1024 / kNarrowLanes;
+    p.block = dim3(kNarrowLanes, workers, 1);
+    p.smem = two_pass_smem(n, kNarrowLanes, 1);
   }
   return p;
 }
-
-constexpr size_t kMaxSmem = 227 * 1024;
 
 template <typename K>
 int set_smem(K kernel, size_t bytes) {
@@ -334,17 +358,20 @@ int set_smem(K kernel, size_t bytes) {
   return FFCB_OK;
 }
 
-#define FFCB_DISPATCH_N(PLAN, ...)                      \
-  switch ((PLAN).N) {                                   \
-    case 0: { constexpr int NN = 0; __VA_ARGS__; } break;      \
-    case 4: { constexpr int NN = 4; __VA_ARGS__; } break;      \
-    case 8: { constexpr int NN = 8; __VA_ARGS__; } break;      \
-    case 16: { constexpr int NN = 16; __VA_ARGS__; } break;    \
-    case 32: { constexpr int NN = 32; __VA_ARGS__; } break;    \
-    case 64: { constexpr int NN = 64; __VA_ARGS__; } break;    \
-    case 128: { constexpr int NN = 128; __VA_ARGS__; } break;  \
-    case 256: { constexpr int NN = 256; __VA_ARGS__; } break;  \
-    default: set_error("fft: internal plan error"); return FFCB_EINVAL; \
+// NN: template length, LL: channels per CTA
+#define FFCB_DISPATCH_N(PLAN, ...)                                                    \
+  if ((PLAN).lanes == kNarrowLanes) {                                                 \
+    constexpr int NN = 0, LL = kNarrowLanes; __VA_ARGS__;                             \
+  } else switch ((PLAN).N) {                                                          \
+    case 0: { constexpr int NN = 0, LL = kLanes; __VA_ARGS__; } break;                \
+    case 4: { constexpr int NN = 4, LL = kLanes; __VA_ARGS__; } break;                \
+    case 8: { constexpr int NN = 8, LL = kLanes; __VA_ARGS__; } break;                \
+    case 16: { constexpr int NN = 16, LL = kLanes; __VA_ARGS__; } break;              \
+    case 32: { constexpr int NN = 32, LL = kLanes; __VA_ARGS__; } break;              \
+    case 64: { constexpr int NN = 64, LL = kLanes; __VA_ARGS__; } break;              \
+    case 128: { constexpr int NN = 128, LL = kLanes; __VA_ARGS__; } break;            \
+    case 256: { constexpr int NN = 256, LL = kLanes; __VA_ARGS__; } break;            \
+    default: set_error("fft: internal plan error"); return FFCB_EINVAL;               \
   }
 
 int check_fft_shapes(const ffcb_tensor* real, const ffcb_tensor* spec, const char* who) {
@@ -352,9 +379,8 @@ int check_fft_shapes(const ffcb_tensor* real, const ffcb_tensor* spec, const cha
   FFCB_REQUIRE(spec->B == real->B && spec->H == real->H && spec->W == real->W / 2 + 1 && spec->C == 2 * real->C,
                "%s: spectrum view must be (B,H,W/2+1,2C) = (%d,%d,%d,%d), got (%d,%d,%d,%d)", who, real->B, real->H,
                real->W / 2 + 1, 2 * real->C, spec->B, spec->H, spec->W, spec->C);
-  LaunchPlan pw = make_plan(real->W), ph = make_plan(real->H);
-  FFCB_REQUIRE(pw.smem <= kMaxSmem && ph.smem <= kMaxSmem, "%s: plane %dx%d exceeds the shared-memory FFT limits",
-               who, real->H, real->W);
+  FFCB_REQUIRE(real->H <= kMaxLen && real->W <= kMaxLen, "%s: plane %dx%d exceeds the %d-point FFT limit", who,
+               real->H, real->W, kMaxLen);
   return FFCB_OK;
 }
 
@@ -392,25 +418,25 @@ int rfft2(const ffcb_tensor* in, const ffcb_tensor* spec, void* ws, size_t ws_by
   if (plane64_eligible(in) && !getenv("FFCB_FFT_TWO_PASS")) return rfft2_plane64(in, spec, stream);
   const View vin = make_view(*in), vspec = make_view(*spec);
   float2* w2 = reinterpret_cast<float2*>(ws);
-  const int cblocks = (in->C + kLanes - 1) / kLanes;
+  const int C = in->C;
   const float scale = (float)(1.0 / sqrt((double)in->H * (double)in->W));
   {
     LaunchPlan p = make_plan(in->W);
     const int pairs = in->B * ((in->H + 1) / 2);
-    dim3 grid((pairs + p.block.z - 1) / p.block.z, cblocks);
+    dim3 grid((pairs + p.block.z - 1) / p.block.z, (C + p.lanes - 1) / p.lanes);
     FFCB_DISPATCH_N(p, {
-      if ((rc = set_smem(rfft_rows_kernel<NN>, p.smem))) return rc;
-      rfft_rows_kernel<NN><<<grid, p.block, p.smem, stream>>>(vin, w2, p.n, p.rp);
+      if ((rc = set_smem(rfft_rows_kernel<NN, LL>, p.smem))) return rc;
+      rfft_rows_kernel<NN, LL><<<grid, p.block, p.smem, stream>>>(vin, w2, p.n, p.rp);
     });
     FFCB_LAUNCH_CHECK("rfft_rows_kernel");
   }
   {
     LaunchPlan p = make_plan(in->H);
     const int cols = in->B * spec->W;
-    dim3 grid((cols + p.block.z - 1) / p.block.z, cblocks);
+    dim3 grid((cols + p.block.z - 1) / p.block.z, (C + p.lanes - 1) / p.lanes);
     FFCB_DISPATCH_N(p, {
-      if ((rc = set_smem(fft_cols_fwd_kernel<NN>, p.smem))) return rc;
-      fft_cols_fwd_kernel<NN><<<grid, p.block, p.smem, stream>>>(w2, vspec, p.n, in->C, scale, p.rp);
+      if ((rc = set_smem(fft_cols_fwd_kernel<NN, LL>, p.smem))) return rc;
+      fft_cols_fwd_kernel<NN, LL><<<grid, p.block, p.smem, stream>>>(w2, vspec, p.n, in->C, scale, p.rp);
     });
     FFCB_LAUNCH_CHECK("fft_cols_fwd_kernel");
   }
@@ -445,25 +471,25 @@ int irfft2(const ffcb_tensor* spec, const ffcb_tensor* residual, const ffcb_tens
     return irfft2_plane64(spec, residual, out, stream);
   const View vspec = make_view(*spec), vout = make_view(*out);
   float2* w2 = reinterpret_cast<float2*>(ws);
-  const int cblocks = (out->C + kLanes - 1) / kLanes;
+  const int C = out->C;
   const float scale = (float)(1.0 / sqrt((double)out->H * (double)out->W));
   {
     LaunchPlan p = make_plan(out->H);
     const int cols = out->B * spec->W;
-    dim3 grid((cols + p.block.z - 1) / p.block.z, cblocks);
+    dim3 grid((cols + p.block.z - 1) / p.block.z, (C + p.lanes - 1) / p.lanes);
     FFCB_DISPATCH_N(p, {
-      if ((rc = set_smem(fft_cols_inv_kernel<NN>, p.smem))) return rc;
-      fft_cols_inv_kernel<NN><<<grid, p.block, p.smem, stream>>>(vspec, w2, p.n, out->C, p.rp);
+      if ((rc = set_smem(fft_cols_inv_kernel<NN, LL>, p.smem))) return rc;
+      fft_cols_inv_kernel<NN, LL><<<grid, p.block, p.smem, stream>>>(vspec, w2, p.n, out->C, p.rp);
     });
     FFCB_LAUNCH_CHECK("fft_cols_inv_kernel");
   }
   {
     LaunchPlan p = make_plan(out->W);
     const int pairs = out->B * ((out->H + 1) / 2);
-    dim3 grid((pairs + p.block.z - 1) / p.block.z, cblocks);
+    dim3 grid((pairs + p.block.z - 1) / p.block.z, (C + p.lanes - 1) / p.lanes);
     FFCB_DISPATCH_N(p, {
-      if ((rc = set_smem(irfft_rows_kernel<NN>, p.smem))) return rc;
-      irfft_rows_kernel<NN><<<grid, p.block, p.smem, stream>>>(w2, vres, vout, p.n, scale, p.rp);
+      if ((rc = set_smem(irfft_rows_kernel<NN, LL>, p.smem))) return rc;
+      irfft_rows_kernel<NN, LL><<<grid, p.block, p.smem, stream>>>(w2, vres, vout, p.n, scale, p.rp);
     });
     FFCB_LAUNCH_CHECK("irfft_rows_kernel");
   }

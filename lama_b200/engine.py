@@ -482,12 +482,13 @@ def _plain_conv(conv, k_ok=(1, 3, 7)) -> bool:
             and conv.in_channels % 4 == 0 and conv.out_channels % 4 == 0)
 
 
+FFT_MAX_LEN = 1024
+
+
 def fft_len_ok(n: int) -> bool:
-    """Lengths the shared-memory FFT kernels take (csrc/fft.cu: make_plan / kMaxSmem): powers of two up to 256 have
-    compile-time plans; any other length needs 8 * (n + 2 * n * 32) bytes of shared memory <= 227 KB, i.e. n <= 446."""
-    if n >= 4 and (n & (n - 1)) == 0:
-        return n <= 256
-    return 1 <= n and 8 * (n + 64 * n) <= 227 * 1024
+    """Lengths the shared-memory FFT kernels take (csrc/fft.cu: make_plan, check_fft_shapes): every length 1 .. 1024.
+    Lengths up to 447 run 32 channels per CTA, 448 .. 1024 (the bottlenecks of 4K-class photos) 8 channels per CTA."""
+    return 1 <= n <= FFT_MAX_LEN
 
 
 def plane_ok(h: int, w: int) -> bool:
@@ -625,7 +626,7 @@ def generator_supported(gen, x) -> bool:
     f = 2 ** len(downs)
     if h % f or w % f:                      # ConvTranspose doubles sizes: only exact multiples round-trip
         return False
-    if blocks_use_fft(gen) and not plane_ok(h // f, w // f):     # e.g. 512-wide bottleneck planes (4096 px images)
+    if blocks_use_fft(gen) and not plane_ok(h // f, w // f):     # e.g. 1025-wide planes (images above 8192 px)
         return False
     return h // f >= 2 and w // f >= 2      # reflect pad 1 at the bottleneck
 
@@ -1644,6 +1645,14 @@ def invalidate(module) -> None:
     checks cannot see; load_state_dict, .to(), in-place ops and ``.data`` edits ARE seen)."""
     _PROGRAMS.pop(module, None)
     _TENSORS.pop(module, None)
+
+
+def drop_executor(ex: "CudaExecutor") -> None:
+    """Remove ``ex`` from every module's executor cache, so that its buffers are freed once the caller lets go of it
+    (a pipeline that releases its program to make room for another)."""
+    for cache in list(_PROGRAMS.values()):
+        for k in [k for k, v in cache.items() if v[1] is ex]:
+            del cache[k]
 
 
 def _content_checksum(tensors) -> float:

@@ -20,7 +20,9 @@ There is no CPU path: a generator that is not on a CUDA device, or is outside th
 from __future__ import annotations
 
 import argparse
+import gc
 import glob
+import logging
 import os
 from collections import OrderedDict
 from typing import Dict, Iterable, List, Optional, Sequence, Tuple
@@ -30,22 +32,33 @@ import torch
 
 from .serving import GeneratorPipeline
 
+log = logging.getLogger(__name__)
+
 
 class BatchedInpainter:
     """Groups equally sized (image, mask) pairs into batches and runs them through u8 generator pipelines.
 
     One pipeline (program + CUDA graph + staging buffers) is kept per (batch, H0, W0); the least recently used
-    one is dropped when more than ``max_pipelines`` shapes are alive (a 512x512 bs32 program holds ~10 GB)."""
+    one is dropped when more than ``max_pipelines`` shapes are alive (a 512x512 bs32 program holds ~10 GB).
+
+    Batches are sized to fit ``mem_budget``: the device bytes the alive pipelines may pool (default: 70 % of the free
+    device memory, plus what this inpainter's own pipelines hold, when a group of equally sized images starts).  A
+    group whose ``max_batch`` images fit runs in batches of ``max_batch``; a larger one (big-lama on a 4K photo holds
+    ~8 GB per image) is cut into balanced batches of the most images that fit.  Pipelines of another shape are released
+    before one that would not fit beside them is built.  An image that alone exceeds the budget still runs at batch 1:
+    if it does not fit the device, the allocation error surfaces."""
 
     def __init__(self, generator, max_batch: int = 32, pad_mod: int = 8, device: Optional[torch.device] = None,
-                 max_pipelines: int = 2, depth: int = 2):
+                 max_pipelines: int = 2, depth: int = 2, mem_budget: Optional[int] = None):
         self.generator = generator.eval()
         self.device = device if device is not None else next(generator.parameters()).device
         if self.device.type != "cuda":
             raise RuntimeError("BatchedInpainter needs the generator on a CUDA device (there is no CPU path)")
         self.max_batch, self.pad_mod, self.depth = int(max_batch), int(pad_mod), int(depth)
         self.max_pipelines = max_pipelines
+        self.mem_budget = mem_budget
         self._pipes: "OrderedDict[Tuple[int, int, int], _Lane]" = OrderedDict()
+        self._per_image: Dict[Tuple[int, int], int] = {}
 
     # -- planning (pure host logic, unit-tested on CPU)
     @staticmethod
@@ -61,16 +74,73 @@ class BatchedInpainter:
                 out.append((hw, idx[k:k + max_batch]))
         return out
 
-    def _lane(self, b: int, h0: int, w0: int) -> "_Lane":
+    @staticmethod
+    def plan_group(idx: Sequence[int], per_image_bytes: int, budget: int, max_batch: int) -> List[List[int]]:
+        """Batches of one group of equally sized images: those of ``plan`` when ``max_batch`` images fit ``budget``,
+        else balanced batches of at most ``budget // per_image_bytes`` images (at least one)."""
+        from .refine import BatchedRefiner
+        if int(budget) // max(1, int(per_image_bytes)) >= max_batch:
+            return [list(idx[k:k + max_batch]) for k in range(0, len(idx), max_batch)]
+        return BatchedRefiner.plan_batches(idx, per_image_bytes, budget, max_batch)
+
+    def per_image_bytes(self, h0: int, w0: int) -> int:
+        """Device bytes of one image's share of a pipeline at (h0, w0): the activations, workspace and outputs of the
+        one-image ``generator_u8`` program (``engine.program_storage_bytes``; a program of B images pools at most B
+        times this), plus the pipeline's device staging (``depth`` input and output slots, the graph's static input)."""
+        key = (int(h0), int(w0))
+        if key not in self._per_image:
+            from . import engine as E
+            metas = (torch.empty(1, h0, w0, 3, dtype=torch.uint8, device="meta"),
+                     torch.empty(1, h0, w0, dtype=torch.uint8, device="meta"))
+            with torch.no_grad():
+                prog = E.build_module_program(self.generator, f"generator_u8:{self.pad_mod}",
+                                              tuple(tuple(m.shape) for m in metas), E.default_math())
+            staging = (self.depth + 1) * 4 * h0 * w0 + self.depth * 3 * h0 * w0
+            self._per_image[key] = E.program_storage_bytes(prog) + staging
+        return self._per_image[key]
+
+    def _alive_bytes(self) -> int:
+        return sum(lane.bytes for lane in self._pipes.values())
+
+    def _budget(self) -> int:
+        if self.mem_budget is not None:
+            return int(self.mem_budget)
+        return int(0.7 * (torch.cuda.mem_get_info(self.device)[0] + self._alive_bytes()))
+
+    def _release_oldest(self):
+        """Close the least recently used lane and free its device memory.  ``_pipes`` must hold the only reference to
+        it (``inpaint`` keeps none across ``_lane``), so that its buffers are gone before the next lane allocates."""
+        _, old = self._pipes.popitem(last=False)
+        old.close()
+        del old
+        gc.collect()                              # executor / graph objects may sit in reference cycles
+        torch.cuda.empty_cache()
+
+    def _lane(self, b: int, h0: int, w0: int, budget: int) -> "_Lane":
         key = (b, h0, w0)
         lane = self._pipes.pop(key, None)
         if lane is None:
-            while len(self._pipes) >= self.max_pipelines:
-                _, old = self._pipes.popitem(last=False)
-                old.close()
+            need = b * self.per_image_bytes(h0, w0)
+            while self._pipes and (len(self._pipes) >= self.max_pipelines or self._alive_bytes() + need > budget):
+                self._release_oldest()
             lane = _Lane(self.generator, b, h0, w0, self.device, self.depth, self.pad_mod)
+            lane.bytes = need
         self._pipes[key] = lane
         return lane
+
+    def batches(self, sizes: Sequence[Tuple[int, int]]):
+        """Yields ((H0, W0), [indices...], budget): ``plan``'s groups cut by ``plan_group`` under the budget taken
+        when each group starts."""
+        for hw, idx in self.plan(sizes, max(1, len(sizes))):
+            budget = self._budget()
+            per = self.per_image_bytes(*hw)
+            parts = self.plan_group(idx, per, budget, self.max_batch)
+            if budget // per < self.max_batch:
+                log.info("%dx%d images: %d per batch at most, batches of %s (one image needs %.2f GB of a %.2f GB "
+                         "budget)", hw[0], hw[1], max(1, budget // per), sorted({len(p) for p in parts}, reverse=True),
+                         per / 1e9, budget / 1e9)
+            for part in parts:
+                yield hw, part, budget
 
     @torch.no_grad()
     def inpaint(self, items: Iterable[Tuple[np.ndarray, np.ndarray]]) -> List[np.ndarray]:
@@ -91,19 +161,23 @@ class BatchedInpainter:
                 for j, i in enumerate(idx):
                     results[i] = out[j].copy()
 
-        for (h0, w0), idx in self.plan([im.shape[:2] for im, _ in items], self.max_batch):
+        for (h0, w0), idx, budget in self.batches([im.shape[:2] for im, _ in items]):
             # a partial batch runs at its own size (programs are per shape); full batches share one pipeline
             if inflight and inflight[-1][0].key != (len(idx), h0, w0):
                 collect(0)                        # results live in the lane's buffers: drain before switching
-            lane = self._lane(len(idx), h0, w0)
             collect(self.depth - 1)
-            img_h, mask_h = lane.stage()
-            for j, i in enumerate(idx):
-                img_h[j].copy_(torch.from_numpy(np.ascontiguousarray(items[i][0])))
-                mask_h[j].copy_(torch.from_numpy(np.ascontiguousarray(items[i][1])))
-            inflight.append((lane, lane.pipe.submit(img_h, mask_h), idx))
+            # no local reference to a lane survives the loop body: a lane _lane releases must be unreachable
+            inflight.append(self._submit(self._lane(len(idx), h0, w0, budget), idx, items))
         collect(0)
         return results  # type: ignore[return-value]
+
+    @staticmethod
+    def _submit(lane: "_Lane", idx: List[int], items) -> Tuple["_Lane", int, List[int]]:
+        img_h, mask_h = lane.stage()
+        for j, i in enumerate(idx):
+            img_h[j].copy_(torch.from_numpy(np.ascontiguousarray(items[i][0])))
+            mask_h[j].copy_(torch.from_numpy(np.ascontiguousarray(items[i][1])))
+        return lane, lane.pipe.submit(img_h, mask_h), idx
 
     def __call__(self, images: np.ndarray, masks: np.ndarray) -> np.ndarray:
         """Equally sized batch: images (B,H,W,3) uint8, masks (B,H,W) uint8 -> (B,H,W,3) uint8."""
@@ -116,6 +190,7 @@ class _Lane:
 
     def __init__(self, generator, b, h0, w0, device, depth, pad_mod):
         self.key = (b, h0, w0)
+        self.bytes = 0
         self.pipe = GeneratorPipeline(generator, b, h0, w0, device=device, depth=depth, u8=True, pad_mod=pad_mod)
         self._stage = [(torch.empty((b, h0, w0, 3), dtype=torch.uint8).pin_memory(),
                         torch.empty((b, h0, w0), dtype=torch.uint8).pin_memory()) for _ in range(depth + 1)]
@@ -127,7 +202,11 @@ class _Lane:
         return pair
 
     def close(self):
+        """Wait for the pipeline's work and drop its executor from the generator's program cache, so that its buffers
+        are freed with the lane."""
+        from . import engine as E
         self.pipe.drain()
+        E.drop_executor(self.pipe.ex)
 
 
 # ------------------------------------------------------------------------------- checkpoint / files
@@ -202,7 +281,7 @@ def build_parser() -> argparse.ArgumentParser:
     ap.add_argument("--img-suffix", default=".png")
     ap.add_argument("--out-ext", default=".png")
     ap.add_argument("--batch", type=int, default=32,
-                    help="images per batch (with --refine: the most; smaller when the step program would not fit)")
+                    help="images per batch at most; smaller when the programs would not fit device memory")
     ap.add_argument("--pad-mod", type=int, default=8, help="pad to a multiple of this (the refiner's modulo too)")
     # configs/prediction/default.yaml: refine, refiner.{n_iters, lr, min_side, max_scales, px_budget}
     ap.add_argument("--refine", action="store_true",
@@ -224,6 +303,7 @@ def refiner_kwargs(a: argparse.Namespace) -> Dict:
 
 def main(argv=None):
     a = build_parser().parse_args(argv)
+    logging.basicConfig(level=logging.INFO, format="%(message)s")
     # one process per GPU (python -m torch.distributed.run --nproc-per-node N -m lama_b200.predict ...): every rank
     # takes its share of the files; single-process runs see rank 0 of 1
     rank, world = int(os.environ.get("RANK", "0")), int(os.environ.get("WORLD_SIZE", "1"))
