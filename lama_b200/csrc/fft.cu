@@ -13,7 +13,9 @@
 // Sizes: power-of-two lengths 4..256 run a mixed-radix (8/4) Stockham autosort (ping-pong buffers);
 // every other length runs the runtime mixed-radix Stockham (a direct DFT for primes), so odd /
 // non-power-of-two planes (bin/predict.py pads images to multiples of 8 only -> e.g. 125x188
-// bottlenecks) stay native.
+// bottlenecks) stay native.  Lengths with a large prime factor (e.g. 479), where that plan costs
+// nearly n^2, run a Bluestein chirp-z transform through compile-time radix-8/4 passes of the power of
+// two m >= 2n - 1 (fft_core.cuh: make_bluestein_plan), 8 or 4 channels per CTA (setup_tile).
 //
 // Channels per CTA (template L): 32, or 8 for lengths 448..1024, whose 32-channel ping-pong buffers
 // (8 * (n + 64 n) bytes) exceed the 227 KB of shared memory a CTA may hold; the 8-channel CTA needs
@@ -30,32 +32,77 @@ namespace ffcb {
 namespace {
 
 constexpr int kLanes = 32;        // channels per CTA of every length whose buffers fit
-constexpr int kNarrowLanes = 8;   // channels per CTA of lengths 448..1024
+constexpr int kNarrowLanes = 8;   // channels per CTA of lengths 448..1024, and of Bluestein lengths up to n = 512
+constexpr int kBsWideLanes = 4;   // channels per CTA of Bluestein lengths 513..1024 (2048-long buffers: fft_core.cuh)
 constexpr int kMaxLen = 1024;     // longest axis (make_rt_plan factors every length up to 1024)
 using namespace fftc;
 
-// Complex FFT of length N (compile-time power of two, or runtime n when N == 0) for this lane.
-// `a` holds the input (already synchronised), `b` is scratch of the same size; returns the
-// buffer holding the result.  Ends with a barrier.
-template <int N, int L, bool INV>
-__device__ __forceinline__ float2* fft_dispatch(float2* a, float2* b, const float2* tw, int n, int lane, int worker,
-                                                int nworkers, const RtPlan& rp) {
-  if constexpr (N == 0) {
+// Runtime mixed-radix Stockham (row f2) of length n for this lane: `a` holds the input (already synchronised), `b`
+// is scratch of the same size; returns the buffer holding the result.  Ends with a barrier.
+template <bool INV, int LS>
+__device__ __forceinline__ float2* rt_passes(float2* a, float2* b, const float2* tw, int n, const RtPlan& rp, int lane,
+                                             int worker, int nworkers) {
+  int ns = 1;
+  for (int p = 0; p < rp.np; ++p) {
+    const int R = rp.radix[p];
+    generic_pass<INV, LS>(a, b, tw, n, R, ns, lane, worker, nworkers);
+    __syncthreads();
+    ns *= R;
+    float2* t = a; a = b; b = t;
+  }
+  return a;
+}
+
+// Compile-time Stockham passes PASS.. of length N (a Bluestein convolution length) from `a`, scratch `b`; returns the
+// buffer holding the result.  Each pass ends with a barrier.
+template <int N, int PASS, bool INV, int LS>
+__device__ __forceinline__ float2* stockham_passes(float2* a, float2* b, const float2* tw, int lane, int worker,
+                                                   int nworkers) {
+  if constexpr (PASS == Plan<N>::P) {
+    return a;
+  } else {
+    stockham_pass<N, PASS, INV, LS>(a, b, tw, lane, worker, nworkers);
+    __syncthreads();
+    return stockham_passes<N, PASS + 1, INV, LS>(b, a, tw, lane, worker, nworkers);
+  }
+}
+
+// Shared-memory tile of one CTA.  Two-pass: [twiddles n][group g: ping n*L | pong n*L].
+// Bluestein: [twiddles m][chirp n][filter spectrum m][ping m*L | pong m*L] (one group).
+struct Tile {
+  float2* tw;
+  float2* data;    // the kernel stages its n input points here
+  float2* tmp;
+  float2* chirp;   // Bluestein only
+  float2* filt;    // Bluestein only
+};
+
+// Complex FFT of length N (compile-time power of two, or runtime n when N == 0) for this lane on t.data (already
+// synchronised); returns the buffer holding the n results in natural order.  BM > 0: Bluestein through BM-point
+// compile-time transforms (fft_core.cuh); otherwise rp is the plan of n.  Ends with a barrier.
+template <int N, int L, bool INV, int BM>
+__device__ __forceinline__ float2* fft_dispatch(const Tile& t, int n, int lane, int worker, int nworkers,
+                                                const RtPlan& rp) {
+  float2 *a = t.data, *b = t.tmp;
+  if constexpr (BM > 0) {                  // Bluestein (chirp-z)
+    bluestein_pre<L>(a, t.chirp, n, BM, lane, worker, nworkers);
+    __syncthreads();
+    float2* f = stockham_passes<BM, 0, false, L>(a, b, t.tw, lane, worker, nworkers);
+    bluestein_mul<L>(f, t.filt, BM, lane, worker, nworkers);
+    __syncthreads();
+    float2* g = stockham_passes<BM, 0, true, L>(f, f == a ? b : a, t.tw, lane, worker, nworkers);
+    bluestein_post<L>(g, t.chirp, n, lane, worker, nworkers);
+    __syncthreads();
+    return g;
+  } else if constexpr (N == 0) {
     if (rp.np < 0) {                       // direct DFT
-      dft_pass<INV, L>(a, b, tw, n, lane, worker, nworkers);
+      dft_pass<INV, L>(a, b, t.tw, n, lane, worker, nworkers);
       __syncthreads();
       return b;
     }
-    int ns = 1;                            // runtime mixed-radix Stockham (row f2)
-    for (int p = 0; p < rp.np; ++p) {
-      const int R = rp.radix[p];
-      generic_pass<INV, L>(a, b, tw, n, R, ns, lane, worker, nworkers);
-      __syncthreads();
-      ns *= R;
-      float2* t = a; a = b; b = t;
-    }
-    return a;
+    return rt_passes<INV, L>(a, b, t.tw, n, rp, lane, worker, nworkers);   // runtime mixed-radix Stockham
   } else {
+    const float2* tw = t.tw;
     stockham_pass<N, 0, INV, L>(a, b, tw, lane, worker, nworkers);
     __syncthreads();
     if constexpr (Plan<N>::P == 1) return b;
@@ -82,25 +129,50 @@ __device__ __forceinline__ void make_twiddles(float2* tw, int n) {
   }
 }
 
-// Shared-memory carve-up: [twiddles n][group g: ping n*L | pong n*L]
-template <int N, int L>
-__device__ __forceinline__ void carve(float2* smem, int n, int group, float2*& tw, float2*& data, float2*& tmp) {
-  tw = smem;
-  data = smem + n + (size_t)group * 2 * n * L;
-  tmp = data + n * L;
+// Carves this group's tile out of shared memory and fills the tables: twiddles of the transform length (m for
+// Bluestein), and for Bluestein the chirp of direction INV and the filter spectrum FFT_m(h) / m, which every thread of
+// the CTA computes together with the m-point passes, using the ping buffer as scratch (the caller stages its input
+// only afterwards).  Ends with a barrier when it wrote more than the twiddles (the kernels' staging loops end with one).
+template <int N, int L, bool INV, int BM>
+__device__ __forceinline__ Tile setup_tile(float2* smem, int n, int group) {
+  Tile t;
+  if constexpr (BM > 0) {
+    constexpr int m = BM;
+    t.tw = smem;
+    t.chirp = smem + m;
+    t.filt = t.chirp + n;
+    t.data = t.filt + m;
+    t.tmp = t.data + (size_t)m * L;
+    make_twiddles(t.tw, m);
+    const int tid = threadIdx.x + blockDim.x * (threadIdx.y + blockDim.y * threadIdx.z);
+    const int nthreads = blockDim.x * blockDim.y * blockDim.z;
+    for (int j = tid; j < n; j += nthreads) t.chirp[j] = bluestein_chirp<INV>(j, n);
+    for (int j = tid; j < m; j += nthreads) t.filt[j] = bluestein_filter<INV>(j, n, m);
+    __syncthreads();
+    const float2* f = stockham_passes<m, 0, false, 1>(t.filt, t.data, t.tw, 0, tid, nthreads);
+    const float inv_m = 1.0f / (float)m;
+    for (int j = tid; j < m; j += nthreads) t.filt[j] = cscale(f[j], inv_m);
+    __syncthreads();
+  } else {
+    t.tw = smem;
+    t.data = smem + n + (size_t)group * 2 * n * L;
+    t.tmp = t.data + n * L;
+    t.chirp = t.filt = nullptr;
+    make_twiddles(t.tw, n);
+  }
+  return t;
 }
 
 // ---------------------------------------------------------------------------------------------
 // Row pass, forward.  grid.x = ceil(B*ceil(H/2) / G), grid.y = ceil(C/L).
 // in (B,H,W,C) real  ->  ws[b][y][k][c] complex, k = 0..W/2   (unscaled)
-template <int N, int L>
+template <int N, int L, int BM>
 __global__ void __launch_bounds__(1024) rfft_rows_kernel(View in, float2* __restrict__ ws, int n, RtPlan rp) {
   extern __shared__ float2 smem_f2[];
   const int W = (N > 0) ? N : n;
   const int lane = threadIdx.x, worker = threadIdx.y, nworkers = blockDim.y, group = threadIdx.z;
-  float2 *tw, *data, *tmp;
-  carve<N, L>(smem_f2, W, group, tw, data, tmp);
-  make_twiddles(tw, W);
+  const Tile t = setup_tile<N, L, false, BM>(smem_f2, W, group);
+  float2* data = t.data;
 
   const int hp = (in.H + 1) / 2;
   const int pair = blockIdx.x * blockDim.z + group;       // (b, y-pair)
@@ -120,7 +192,7 @@ __global__ void __launch_bounds__(1024) rfft_rows_kernel(View in, float2* __rest
     data[x * L + lane] = z;
   }
   __syncthreads();
-  const float2* res = fft_dispatch<N, L, false>(data, tmp, tw, W, lane, worker, nworkers, rp);
+  const float2* res = fft_dispatch<N, L, false, BM>(t, W, lane, worker, nworkers, rp);
 
   const int wf = W / 2 + 1;
   if (cok) {
@@ -136,15 +208,14 @@ __global__ void __launch_bounds__(1024) rfft_rows_kernel(View in, float2* __rest
 
 // Column pass, forward.  grid.x = ceil(B*Wf / G), grid.y = ceil(C/L).
 // ws[b][y][k][c] complex -> spec (B,H,Wf,2C): channel 2c = Re, 2c+1 = Im, scaled by `scale`.
-template <int N, int L>
+template <int N, int L, int BM>
 __global__ void __launch_bounds__(1024) fft_cols_fwd_kernel(const float2* __restrict__ ws, View spec, int n,
                                                             int C, float scale, RtPlan rp) {
   extern __shared__ float2 smem_f2[];
   const int H = (N > 0) ? N : n;
   const int lane = threadIdx.x, worker = threadIdx.y, nworkers = blockDim.y, group = threadIdx.z;
-  float2 *tw, *data, *tmp;
-  carve<N, L>(smem_f2, H, group, tw, data, tmp);
-  make_twiddles(tw, H);
+  const Tile t = setup_tile<N, L, false, BM>(smem_f2, H, group);
+  float2* data = t.data;
 
   const int wf = spec.W;
   const int col = blockIdx.x * blockDim.z + group;  // (b, k)
@@ -160,7 +231,7 @@ __global__ void __launch_bounds__(1024) fft_cols_fwd_kernel(const float2* __rest
     data[y * L + lane] = z;
   }
   __syncthreads();
-  const float2* res = fft_dispatch<N, L, false>(data, tmp, tw, H, lane, worker, nworkers, rp);
+  const float2* res = fft_dispatch<N, L, false, BM>(t, H, lane, worker, nworkers, rp);
 
   if (cok) {
     for (int y = worker; y < H; y += nworkers) {
@@ -182,14 +253,13 @@ __global__ void __launch_bounds__(1024) fft_cols_fwd_kernel(const float2* __rest
 }
 
 // Column pass, inverse: spec (B,H,Wf,2C) -> ws[b][y][k][c] complex (unscaled inverse along H).
-template <int N, int L>
+template <int N, int L, int BM>
 __global__ void __launch_bounds__(N > 0 && N <= 64 ? 256 : 1024, N > 0 && N <= 64 ? 6 : 1) fft_cols_inv_kernel(View spec, float2* __restrict__ ws, int n, int C, RtPlan rp) {
   extern __shared__ float2 smem_f2[];
   const int H = (N > 0) ? N : n;
   const int lane = threadIdx.x, worker = threadIdx.y, nworkers = blockDim.y, group = threadIdx.z;
-  float2 *tw, *data, *tmp;
-  carve<N, L>(smem_f2, H, group, tw, data, tmp);
-  make_twiddles(tw, H);
+  const Tile t = setup_tile<N, L, true, BM>(smem_f2, H, group);
+  float2* data = t.data;
 
   const int wf = spec.W;
   const int col = blockIdx.x * blockDim.z + group;
@@ -213,7 +283,7 @@ __global__ void __launch_bounds__(N > 0 && N <= 64 ? 256 : 1024, N > 0 && N <= 6
     data[y * L + lane] = z;
   }
   __syncthreads();
-  const float2* res = fft_dispatch<N, L, true>(data, tmp, tw, H, lane, worker, nworkers, rp);
+  const float2* res = fft_dispatch<N, L, true, BM>(t, H, lane, worker, nworkers, rp);
 
   if (cok) {
     for (int y = worker; y < H; y += nworkers)
@@ -223,15 +293,14 @@ __global__ void __launch_bounds__(N > 0 && N <= 64 ? 256 : 1024, N > 0 && N <= 6
 
 // Row pass, inverse (C2R, two rows at a time): ws[b][y][k][c] -> out (B,H,W,C) real,
 // out = residual + scale * c2r(ws).  Im of bins 0 and (even W) W/2 is ignored.
-template <int N, int L>
+template <int N, int L, int BM>
 __global__ void __launch_bounds__(N > 0 && N <= 64 ? 256 : 1024, N > 0 && N <= 64 ? 6 : 1) irfft_rows_kernel(const float2* __restrict__ ws, View res, View out, int n,
                                                           float scale, RtPlan rp) {
   extern __shared__ float2 smem_f2[];
   const int W = (N > 0) ? N : n;
   const int lane = threadIdx.x, worker = threadIdx.y, nworkers = blockDim.y, group = threadIdx.z;
-  float2 *tw, *data, *tmp;
-  carve<N, L>(smem_f2, W, group, tw, data, tmp);
-  make_twiddles(tw, W);
+  const Tile t = setup_tile<N, L, true, BM>(smem_f2, W, group);
+  float2* data = t.data;
 
   const int hp = (out.H + 1) / 2;
   const int pair = blockIdx.x * blockDim.z + group;
@@ -253,7 +322,7 @@ __global__ void __launch_bounds__(N > 0 && N <= 64 ? 256 : 1024, N > 0 && N <= 6
     c2r_pair_pre<L>(data, W, k, lane, x1, x2);
   }
   __syncthreads();
-  const float2* fin = fft_dispatch<N, L, true>(data, tmp, tw, W, lane, worker, nworkers, rp);
+  const float2* fin = fft_dispatch<N, L, true, BM>(t, W, lane, worker, nworkers, rp);
 
   if (cok) {
     if (N > 0) {
@@ -295,22 +364,33 @@ __global__ void __launch_bounds__(N > 0 && N <= 64 ? 256 : 1024, N > 0 && N <= 6
 struct LaunchPlan {
   int N;       // template length (0 = runtime length)
   int n;       // runtime length
-  int lanes;   // channels per CTA: kLanes, or kNarrowLanes (N == 0 only)
+  int m;       // Bluestein convolution length: 512, 1024 or 2048 (n otherwise)
+  bool bluestein;
+  int lanes;   // channels per CTA: kLanes, or kNarrowLanes (N == 0 only); Bluestein: kNarrowLanes or kBsWideLanes
   dim3 block;  // (lanes, workers, groups)
   size_t smem;
-  RtPlan rp;   // N == 0: runtime radix plan (np < 0: direct DFT)
+  RtPlan rp;   // N == 0 without Bluestein: runtime radix plan (np < 0: direct DFT)
 };
 
 // Lengths without a compile-time plan: runtime mixed-radix Stockham (FFCB_FFT_MIXED_RADIX=0 selects the O(n^2)
-// direct DFT they ran in the first revision — same results to round-off, kept as the cross-check).
+// direct DFT they ran in the first revision — same results to round-off, kept as the cross-check; it turns Bluestein
+// off too).
 bool mixed_radix_enabled() {
   const char* e = getenv("FFCB_FFT_MIXED_RADIX");
+  return e ? atoi(e) != 0 : true;
+}
+
+// Lengths with a large prime factor: Bluestein when the planner prices it below the runtime plan
+// (FFCB_FFT_BLUESTEIN=0 restores the runtime plans, kept as the cross-check).
+bool bluestein_enabled() {
+  const char* e = getenv("FFCB_FFT_BLUESTEIN");
   return e ? atoi(e) != 0 : true;
 }
 
 bool is_pow2(int v) { return v > 0 && (v & (v - 1)) == 0; }
 
 constexpr size_t kMaxSmem = 227 * 1024;
+static_assert(kMaxSmem == (size_t)kBluesteinSmemLimit, "one shared-memory limit for the planner and the kernels");
 
 size_t two_pass_smem(int n, int lanes, int groups) {
   return sizeof(float2) * ((size_t)n + (size_t)groups * 2 * n * lanes);
@@ -319,10 +399,26 @@ size_t two_pass_smem(int n, int lanes, int groups) {
 LaunchPlan make_plan(int n) {
   LaunchPlan p;
   p.n = n;
+  p.m = n;
+  p.bluestein = false;
   p.lanes = kLanes;
   p.rp.np = -1;
   for (int i = 0; i < kMaxRtPasses; ++i) p.rp.radix[i] = 1;
-  if (is_pow2(n) && n >= 4 && n <= 256) {
+  BluesteinPlan bp;
+  bp.m = 0;
+  if (!(is_pow2(n) && n >= 4 && n <= 256) && mixed_radix_enabled() && bluestein_enabled())
+    bp = make_bluestein_plan(n);
+  if (bp.m > 0) {
+    // Bluestein: one group of 8 (m = 512, 1024) or 4 (m = 2048) channels, m / 8 workers: one radix-8 butterfly per
+    // worker and pass, up to a full 1024-thread CTA (fft_core.cuh: bluestein_lanes)
+    p.N = 0;
+    p.m = bp.m;
+    p.bluestein = true;
+    p.lanes = bp.lanes;
+    const int workers = (bp.m + 7) / 8 < 1024 / bp.lanes ? (bp.m + 7) / 8 : 1024 / bp.lanes;
+    p.block = dim3(bp.lanes, workers, 1);
+    p.smem = (size_t)bluestein_smem(n, bp.m, bp.lanes);
+  } else if (is_pow2(n) && n >= 4 && n <= 256) {
     p.N = n;
     const int workers = fftc::workers_for(n);
     const int groups = workers >= 8 ? 1 : 8 / workers;
@@ -358,20 +454,27 @@ int set_smem(K kernel, size_t bytes) {
   return FFCB_OK;
 }
 
-// NN: template length, LL: channels per CTA
-#define FFCB_DISPATCH_N(PLAN, ...)                                                    \
-  if ((PLAN).lanes == kNarrowLanes) {                                                 \
-    constexpr int NN = 0, LL = kNarrowLanes; __VA_ARGS__;                             \
-  } else switch ((PLAN).N) {                                                          \
-    case 0: { constexpr int NN = 0, LL = kLanes; __VA_ARGS__; } break;                \
-    case 4: { constexpr int NN = 4, LL = kLanes; __VA_ARGS__; } break;                \
-    case 8: { constexpr int NN = 8, LL = kLanes; __VA_ARGS__; } break;                \
-    case 16: { constexpr int NN = 16, LL = kLanes; __VA_ARGS__; } break;              \
-    case 32: { constexpr int NN = 32, LL = kLanes; __VA_ARGS__; } break;              \
-    case 64: { constexpr int NN = 64, LL = kLanes; __VA_ARGS__; } break;              \
-    case 128: { constexpr int NN = 128, LL = kLanes; __VA_ARGS__; } break;            \
-    case 256: { constexpr int NN = 256, LL = kLanes; __VA_ARGS__; } break;            \
-    default: set_error("fft: internal plan error"); return FFCB_EINVAL;               \
+// NN: template length, LL: channels per CTA, BM: Bluestein convolution length (0: none)
+#define FFCB_DISPATCH_N(PLAN, ...)                                                            \
+  if ((PLAN).bluestein) {                                                                     \
+    switch ((PLAN).m) {                                                                       \
+      case 512: { constexpr int NN = 0, LL = kNarrowLanes, BM = 512; __VA_ARGS__; } break;    \
+      case 1024: { constexpr int NN = 0, LL = kNarrowLanes, BM = 1024; __VA_ARGS__; } break;  \
+      case 2048: { constexpr int NN = 0, LL = kBsWideLanes, BM = 2048; __VA_ARGS__; } break;  \
+      default: set_error("fft: internal plan error"); return FFCB_EINVAL;                     \
+    }                                                                                         \
+  } else if ((PLAN).lanes == kNarrowLanes) {                                                  \
+    constexpr int NN = 0, LL = kNarrowLanes, BM = 0; __VA_ARGS__;                             \
+  } else switch ((PLAN).N) {                                                                  \
+    case 0: { constexpr int NN = 0, LL = kLanes, BM = 0; __VA_ARGS__; } break;                \
+    case 4: { constexpr int NN = 4, LL = kLanes, BM = 0; __VA_ARGS__; } break;                \
+    case 8: { constexpr int NN = 8, LL = kLanes, BM = 0; __VA_ARGS__; } break;                \
+    case 16: { constexpr int NN = 16, LL = kLanes, BM = 0; __VA_ARGS__; } break;              \
+    case 32: { constexpr int NN = 32, LL = kLanes, BM = 0; __VA_ARGS__; } break;              \
+    case 64: { constexpr int NN = 64, LL = kLanes, BM = 0; __VA_ARGS__; } break;              \
+    case 128: { constexpr int NN = 128, LL = kLanes, BM = 0; __VA_ARGS__; } break;            \
+    case 256: { constexpr int NN = 256, LL = kLanes, BM = 0; __VA_ARGS__; } break;            \
+    default: set_error("fft: internal plan error"); return FFCB_EINVAL;                       \
   }
 
 int check_fft_shapes(const ffcb_tensor* real, const ffcb_tensor* spec, const char* who) {
@@ -425,8 +528,8 @@ int rfft2(const ffcb_tensor* in, const ffcb_tensor* spec, void* ws, size_t ws_by
     const int pairs = in->B * ((in->H + 1) / 2);
     dim3 grid((pairs + p.block.z - 1) / p.block.z, (C + p.lanes - 1) / p.lanes);
     FFCB_DISPATCH_N(p, {
-      if ((rc = set_smem(rfft_rows_kernel<NN, LL>, p.smem))) return rc;
-      rfft_rows_kernel<NN, LL><<<grid, p.block, p.smem, stream>>>(vin, w2, p.n, p.rp);
+      if ((rc = set_smem(rfft_rows_kernel<NN, LL, BM>, p.smem))) return rc;
+      rfft_rows_kernel<NN, LL, BM><<<grid, p.block, p.smem, stream>>>(vin, w2, p.n, p.rp);
     });
     FFCB_LAUNCH_CHECK("rfft_rows_kernel");
   }
@@ -435,8 +538,8 @@ int rfft2(const ffcb_tensor* in, const ffcb_tensor* spec, void* ws, size_t ws_by
     const int cols = in->B * spec->W;
     dim3 grid((cols + p.block.z - 1) / p.block.z, (C + p.lanes - 1) / p.lanes);
     FFCB_DISPATCH_N(p, {
-      if ((rc = set_smem(fft_cols_fwd_kernel<NN, LL>, p.smem))) return rc;
-      fft_cols_fwd_kernel<NN, LL><<<grid, p.block, p.smem, stream>>>(w2, vspec, p.n, in->C, scale, p.rp);
+      if ((rc = set_smem(fft_cols_fwd_kernel<NN, LL, BM>, p.smem))) return rc;
+      fft_cols_fwd_kernel<NN, LL, BM><<<grid, p.block, p.smem, stream>>>(w2, vspec, p.n, in->C, scale, p.rp);
     });
     FFCB_LAUNCH_CHECK("fft_cols_fwd_kernel");
   }
@@ -478,8 +581,8 @@ int irfft2(const ffcb_tensor* spec, const ffcb_tensor* residual, const ffcb_tens
     const int cols = out->B * spec->W;
     dim3 grid((cols + p.block.z - 1) / p.block.z, (C + p.lanes - 1) / p.lanes);
     FFCB_DISPATCH_N(p, {
-      if ((rc = set_smem(fft_cols_inv_kernel<NN, LL>, p.smem))) return rc;
-      fft_cols_inv_kernel<NN, LL><<<grid, p.block, p.smem, stream>>>(vspec, w2, p.n, out->C, p.rp);
+      if ((rc = set_smem(fft_cols_inv_kernel<NN, LL, BM>, p.smem))) return rc;
+      fft_cols_inv_kernel<NN, LL, BM><<<grid, p.block, p.smem, stream>>>(vspec, w2, p.n, out->C, p.rp);
     });
     FFCB_LAUNCH_CHECK("fft_cols_inv_kernel");
   }
@@ -488,8 +591,8 @@ int irfft2(const ffcb_tensor* spec, const ffcb_tensor* residual, const ffcb_tens
     const int pairs = out->B * ((out->H + 1) / 2);
     dim3 grid((pairs + p.block.z - 1) / p.block.z, (C + p.lanes - 1) / p.lanes);
     FFCB_DISPATCH_N(p, {
-      if ((rc = set_smem(irfft_rows_kernel<NN, LL>, p.smem))) return rc;
-      irfft_rows_kernel<NN, LL><<<grid, p.block, p.smem, stream>>>(w2, vres, vout, p.n, scale, p.rp);
+      if ((rc = set_smem(irfft_rows_kernel<NN, LL, BM>, p.smem))) return rc;
+      irfft_rows_kernel<NN, LL, BM><<<grid, p.block, p.smem, stream>>>(w2, vres, vout, p.n, scale, p.rp);
     });
     FFCB_LAUNCH_CHECK("irfft_rows_kernel");
   }

@@ -79,10 +79,16 @@ template <> struct Plan<32>  { static constexpr int P = 2; static constexpr int 
 template <> struct Plan<64>  { static constexpr int P = 2; static constexpr int R[3] = {8, 8, 1}; };
 template <> struct Plan<128> { static constexpr int P = 3; static constexpr int R[3] = {8, 4, 4}; };
 template <> struct Plan<256> { static constexpr int P = 3; static constexpr int R[3] = {8, 8, 4}; };
+// convolution lengths of the Bluestein transforms (below)
+template <> struct Plan<512>  { static constexpr int P = 3; static constexpr int R[3] = {8, 8, 8}; };
+template <> struct Plan<1024> { static constexpr int P = 4; static constexpr int R[4] = {8, 8, 4, 4}; };
+template <> struct Plan<2048> { static constexpr int P = 4; static constexpr int R[4] = {8, 8, 8, 4}; };
 
 template <int N, int PASS> constexpr int plan_radix() { return Plan<N>::R[PASS]; }
 template <int N, int PASS> constexpr int plan_ns() {
-  return PASS == 0 ? 1 : (PASS == 1 ? Plan<N>::R[0] : Plan<N>::R[0] * Plan<N>::R[1]);
+  int ns = 1;
+  for (int i = 0; i < PASS; ++i) ns *= Plan<N>::R[i];
+  return ns;
 }
 // worker threads per transform the kernels launch with
 constexpr int workers_for(int n) { return n >= 8 ? n / 8 : 1; }
@@ -228,6 +234,108 @@ FFCB_HD void c2r_pair_pre(float2* z, int W, int k, int lane, float2 x1, float2 x
     z[k * LS + lane] = make_float2(x1.x - x2.y, x1.y + x2.x);          // X1 + i X2
     z[(W - k) * LS + lane] = make_float2(x1.x + x2.y, x2.x - x1.y);    // conj(X1) + i conj(X2)
   }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Bluestein (chirp-z) transforms for runtime lengths with a large prime factor, where the runtime plan above costs
+// nearly n^2.  With c[j] = exp(-+ i pi j^2 / n) (forward / inverse) and jk = (j^2 + k^2 - (k-j)^2) / 2:
+//   X[k] = c[k] * sum_j (x[j] c[j]) conj(c[k-j])
+// a cyclic convolution of the zero-padded chirped input with h[d] = conj(c[|d|]), evaluated at the power of two
+// m >= 2n - 1 (512, 1024 or 2048) as IFFT_m(FFT_m(x c) * FFT_m(h)) / m.  Both m-point transforms run the compile-time
+// radix-8/4 Stockham passes (stockham_pass, Plan<m>): register butterflies with no per-output index arithmetic, which
+// is what makes Bluestein pay off against the runtime plans; a smooth m closer to 2n - 1 would run the generic passes,
+// measured 2-3x slower per point.  The filter spectrum FFT_m(h) / m is the same for every lane: a CTA computes it once.
+struct BluesteinPlan {
+  int m;       // convolution length; 0: the runtime plan of n is cheaper
+  int lanes;   // channels per CTA (bluestein_lanes)
+  float cost;  // modelled cost of the Bluestein transform (0 for lengths it cannot serve)
+  int direct;  // modelled cost of the runtime plan of n
+};
+
+// make_rt_plan's cost model: sum over passes of (R_p + 3) per point
+inline int rt_plan_cost(int n, const RtPlan& p) {
+  if (p.np < 0) return n * (n + 3);
+  int s = 0;
+  for (int i = 0; i < p.np; ++i) s += p.radix[i] + 3;
+  return n * s;
+}
+
+// Shared memory of a Bluestein CTA: [twiddles m][chirp n][filter spectrum m][ping m * lanes | pong m * lanes] float2.
+// 8 channels fit the 227 KB a CTA may hold for m = 512 and 1024 (152 KB at n = 512); m = 2048 takes 4 channels
+// (172 KB at n = 1024), the widest layout that keeps the two m-long buffers per lane the out-of-place passes need.
+constexpr int kBluesteinSmemLimit = 227 * 1024;
+inline int bluestein_smem(int n, int m, int lanes) { return (int)sizeof(float2) * (2 * m + n + 2 * lanes * m); }
+inline int bluestein_lanes(int n, int m) { return bluestein_smem(n, m, 8) <= kBluesteinSmemLimit ? 8 : 4; }
+
+// Bluestein is taken when its modelled cost, times this factor, is below the runtime plan's.  The model prices a
+// compile-time radix-R pass like a runtime one (R + 3 per point), which overstates it; the factor is the measured
+// correction.  tools/fft_lengths_bench.py on an H100 timed every length this factor selects (311 of 129..1024, n x n
+// planes of 192 channels, DESIGN §6): each ran the FFT pair 1.28x to 8.9x faster than its runtime plan.
+constexpr float kBluesteinCostFactor = 0.5f;
+
+// Plan for n: m = 0 when the runtime plan of n stays cheaper.  The model counts two m-point transforms, three
+// point-wise passes (chirp + zero pad over m, filter over m, chirp over n; 4 per point, like a radix-1 pass) and the
+// lane's share of the per-CTA filter transform.  Host only; no search, so it is cheap on every call.
+inline BluesteinPlan make_bluestein_plan(int n) {
+  BluesteinPlan b;
+  b.m = 0;
+  b.lanes = 0;
+  b.cost = 0.f;
+  b.direct = 0;
+  if (n < 129 || n > 1024) return b;                    // m = 512 .. 2048
+  b.direct = rt_plan_cost(n, make_rt_plan(n));
+  int m = 512;
+  while (m < 2 * n - 1) m *= 2;
+  const int per_point = m == 512 ? 3 * (8 + 3) : (m == 1024 ? 2 * (8 + 3) + 2 * (4 + 3) : 3 * (8 + 3) + (4 + 3));
+  const int lanes = bluestein_lanes(n, m);
+  const float tm = (float)m * per_point;
+  b.cost = 2.f * tm + 4.f * (2 * m + n) + tm / lanes;
+  if (kBluesteinCostFactor * b.cost < (float)b.direct) { b.m = m; b.lanes = lanes; }
+  return b;
+}
+
+// c[j] = exp(-+ i pi j^2 / n).  The phase is reduced exactly in integers (j^2 mod 2n) first: j^2 / n in float loses
+// it at n ~ 1000.
+template <bool INV>
+FFCB_HD float2 bluestein_chirp(int j, int n) {
+  const int r = (int)(((long long)j * j) % (2 * n));
+  float s, c;
+#if defined(__CUDA_ARCH__)
+  sincospif((float)r / (float)n, &s, &c);
+#else
+  const double a = M_PI * (double)((float)r / (float)n);
+  s = (float)sin(a);
+  c = (float)cos(a);
+#endif
+  return make_float2(c, INV ? s : -s);
+}
+
+// time-domain filter h[t] = conj(c[t]) for t < n, conj(c[m - t]) for t > m - n, 0 between (m >= 2n - 1)
+template <bool INV>
+FFCB_HD float2 bluestein_filter(int t, int n, int m) {
+  const int d = t < n ? t : (t > m - n ? m - t : -1);
+  if (d < 0) return make_float2(0.f, 0.f);
+  const float2 c = bluestein_chirp<INV>(d, n);
+  return make_float2(c.x, -c.y);
+}
+
+// step 1: a[j] *= c[j] for j < n, zero for n <= j < m (the caller stored points 0..n-1)
+template <int LS>
+FFCB_HD void bluestein_pre(float2* a, const float2* chirp, int n, int m, int lane, int worker, int nworkers) {
+  for (int j = worker; j < m; j += nworkers)
+    a[j * LS + lane] = j < n ? cmul(a[j * LS + lane], chirp[j]) : make_float2(0.f, 0.f);
+}
+
+// step 3: a[k] *= filt[k] (filter spectrum, 1/m folded in), k < m
+template <int LS>
+FFCB_HD void bluestein_mul(float2* a, const float2* filt, int m, int lane, int worker, int nworkers) {
+  for (int k = worker; k < m; k += nworkers) a[k * LS + lane] = cmul(a[k * LS + lane], filt[k]);
+}
+
+// step 5: a[k] *= c[k], k < n: the n results in natural order
+template <int LS>
+FFCB_HD void bluestein_post(float2* a, const float2* chirp, int n, int lane, int worker, int nworkers) {
+  for (int k = worker; k < n; k += nworkers) a[k * LS + lane] = cmul(a[k * LS + lane], chirp[k]);
 }
 
 

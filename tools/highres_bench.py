@@ -2,7 +2,7 @@
 """High-resolution inference of big-lama at batch 1: the native path against the reference's operator sequence under
 torch eager, on 4K-class photos whose bottleneck planes take the 8-channel FFT kernels (448..1024-point axes).
 
-    python tools/highres_bench.py [--sizes 2160x3840,3000x4000,4096x4096,2160x3832] [--steps 10] [--out DIR]
+    python tools/highres_bench.py [--sizes 2160x3840,3000x4000,4096x4096,2160x3832,2160x4016] [--steps 10] [--out DIR]
 
 Per size (the image sides are multiples of 8, so the generator and the predict driver see the same plane):
   * graph_ms      — CUDA-graph replay of the generator program (float in / out), CUDA events over ``--steps`` replays;
@@ -13,7 +13,8 @@ Per size (the image sides are multiples of 8, so the generator and the predict d
   * fft_share     — share of the FFT kernels in the kernel time of one eager program step (every library call issued
                     once), from torch.profiler CUDA activities;
   * max_abs       — (first size only) max |native - CPU fp32 oracle| on the sigmoid output.
-2160x3832 has a prime bottleneck width (479): its rows run the direct DFT.  The card's name and power limit are read
+2160x3832 has a prime bottleneck width (479) and 2160x4016 a width of 502 = 2 * 251 (height 270): both run their rows
+as Bluestein chirp-z transforms (1024-point convolutions).  The card's name and power limit are read
 in the same run and printed with the numbers.  Nothing is written outside ``--out``.
 """
 import argparse
@@ -60,7 +61,7 @@ def fft_share(ex):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--sizes", default="2160x3840,3000x4000,4096x4096,2160x3832")
+    ap.add_argument("--sizes", default="2160x3840,3000x4000,4096x4096,2160x3832,2160x4016")
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--images", type=int, default=4)
     ap.add_argument("--eager-steps", type=int, default=3)
