@@ -892,11 +892,12 @@ def emit_resnet_block(prog: Program, blk, X: Buf, cl: int, cg: int, in_place: bo
     return out
 
 
-# Largest plane side the forward+backward block program is used for: the largest plane its input gradients are tested
-# at against autograd through the oracle (tests/test_gpu_parity.py: 32x32, 64x64, 12x20; tests/test_gpu_program_diff.py:
-# 128x128, 96x128, 256x256 and every op of the program at 128-wide planes).  Larger planes take the torch-autograd
-# composition.
-BLOCK_GRAD_MAX_PLANE = 256
+# Largest plane side the forward+backward block program (and the rear / refinement step programs built on it) is used
+# for: every plane the native FFT pair takes.  Its input gradients are tested against float64 autograd through the
+# oracle from 12x20 up to 256x256 (tests/test_gpu_parity.py, tests/test_gpu_program_diff.py), at 211x251 (Bluestein,
+# tests/test_gpu_fft_bluestein.py) and at 270x480, 259x108 and 128x1024 (8-channel and Bluestein FFT lengths,
+# tests/test_gpu_refine_large_planes.py).  Wider planes are rejected by the FFT kernels and take torch autograd.
+BLOCK_GRAD_MAX_PLANE = FFT_MAX_LEN
 
 
 def block_grad_supported(blk) -> bool:
@@ -1179,7 +1180,7 @@ def rear_grad_supported(gen, shape_l, shape_g) -> bool:
     """The generator's rear — residual blocks, up-sampling tail, head (``generator.model[first_block:]``) — has a
     native forward + input-gradient program for inputs (z1, z2) of these shapes: every block has block gradients
     (``block_grad_supported``), no out_ffc block, at least one up-sampling stage, a none / sigmoid / tanh head with
-    N <= 4, bottleneck planes up to BLOCK_GRAD_MAX_PLANE that the native FFT takes."""
+    N <= 4, bottleneck planes the native FFT takes (``plane_ok``, axes up to BLOCK_GRAD_MAX_PLANE = FFT_MAX_LEN)."""
     lay = _generator_layout(gen)
     if lay is None or shape_l is None or shape_g is None or len(shape_l) != 4 or len(shape_g) != 4:
         return False

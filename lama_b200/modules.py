@@ -320,7 +320,7 @@ class FFCResnetBlock(nn.Module):
         if any(p.requires_grad for p in self.parameters()):
             return False
         if max(x_l.shape[-2:]) > _engine.BLOCK_GRAD_MAX_PLANE:
-            return False            # see engine.BLOCK_GRAD_MAX_PLANE: larger planes take torch autograd
+            return False            # see engine.BLOCK_GRAD_MAX_PLANE: planes the native FFT rejects take torch autograd
         return _engine.block_grad_supported(self) and _engine.ffc_bn_act_shapes_ok(self.conv1, x_l, x_g)
 
     def forward(self, x):

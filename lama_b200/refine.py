@@ -296,11 +296,12 @@ class BatchedRefiner:
 
     Images above ``px_budget`` pixels are refined, and returned, at the reduced size, as by the reference.  Groups whose
     scales the native step program does not cover (``engine.refine_supported``: LFU, out_ffc or gated generators,
-    bottleneck planes above ``engine.BLOCK_GRAD_MAX_PLANE``), and every group under LAMA_B200_NATIVE_GRAD=0, run
+    bottleneck axes above ``engine.FFT_MAX_LEN``), and every group under LAMA_B200_NATIVE_GRAD=0, run
     ``refine_predict`` image by image.  ``mem_budget``: device bytes the programs of one batch, every scale's, may pool
     (default: 70 % of the free device memory when the group starts).  A group is cut into balanced batches, and the
     programs of one batch size are released before those of another are built, so no more than one batch's programs are
-    alive at a time."""
+    alive at a time.  An image whose programs alone exceed the budget still runs, at batch 1; if the device cannot hold
+    them, the allocation error propagates to the caller."""
 
     def __init__(self, generator, max_batch: int = 8, *, modulo: int = 8, n_iters: int = 15, lr: float = 0.002,
                  min_side: int = 512, max_scales: int = 3, px_budget: int = 1800000,
