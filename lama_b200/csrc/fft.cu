@@ -31,8 +31,6 @@
 namespace ffcb {
 namespace {
 
-constexpr int kLanes = 32;        // channels per CTA of every length whose buffers fit
-constexpr int kNarrowLanes = 8;   // channels per CTA of lengths 448..1024, and of Bluestein lengths up to n = 512
 constexpr int kBsWideLanes = 4;   // channels per CTA of Bluestein lengths 513..1024 (2048-long buffers: fft_core.cuh)
 constexpr int kMaxLen = 1024;     // longest axis (make_rt_plan factors every length up to 1024)
 using namespace fftc;
@@ -361,93 +359,7 @@ __global__ void __launch_bounds__(N > 0 && N <= 64 ? 256 : 1024, N > 0 && N <= 6
 }
 
 // ---------------------------------------------------------------------------------------------
-struct LaunchPlan {
-  int N;       // template length (0 = runtime length)
-  int n;       // runtime length
-  int m;       // Bluestein convolution length: 512, 1024 or 2048 (n otherwise)
-  bool bluestein;
-  int lanes;   // channels per CTA: kLanes, or kNarrowLanes (N == 0 only); Bluestein: kNarrowLanes or kBsWideLanes
-  dim3 block;  // (lanes, workers, groups)
-  size_t smem;
-  RtPlan rp;   // N == 0 without Bluestein: runtime radix plan (np < 0: direct DFT)
-};
-
-// Lengths without a compile-time plan: runtime mixed-radix Stockham (FFCB_FFT_MIXED_RADIX=0 selects the O(n^2)
-// direct DFT they ran in the first revision — same results to round-off, kept as the cross-check; it turns Bluestein
-// off too).
-bool mixed_radix_enabled() {
-  const char* e = getenv("FFCB_FFT_MIXED_RADIX");
-  return e ? atoi(e) != 0 : true;
-}
-
-// Lengths with a large prime factor: Bluestein when the planner prices it below the runtime plan
-// (FFCB_FFT_BLUESTEIN=0 restores the runtime plans, kept as the cross-check).
-bool bluestein_enabled() {
-  const char* e = getenv("FFCB_FFT_BLUESTEIN");
-  return e ? atoi(e) != 0 : true;
-}
-
-bool is_pow2(int v) { return v > 0 && (v & (v - 1)) == 0; }
-
-constexpr size_t kMaxSmem = 227 * 1024;
-static_assert(kMaxSmem == (size_t)kBluesteinSmemLimit, "one shared-memory limit for the planner and the kernels");
-
-size_t two_pass_smem(int n, int lanes, int groups) {
-  return sizeof(float2) * ((size_t)n + (size_t)groups * 2 * n * lanes);
-}
-
-LaunchPlan make_plan(int n) {
-  LaunchPlan p;
-  p.n = n;
-  p.m = n;
-  p.bluestein = false;
-  p.lanes = kLanes;
-  p.rp.np = -1;
-  for (int i = 0; i < kMaxRtPasses; ++i) p.rp.radix[i] = 1;
-  BluesteinPlan bp;
-  bp.m = 0;
-  if (!(is_pow2(n) && n >= 4 && n <= 256) && mixed_radix_enabled() && bluestein_enabled())
-    bp = make_bluestein_plan(n);
-  if (bp.m > 0) {
-    // Bluestein: one group of 8 (m = 512, 1024) or 4 (m = 2048) channels, m / 8 workers: one radix-8 butterfly per
-    // worker and pass, up to a full 1024-thread CTA (fft_core.cuh: bluestein_lanes)
-    p.N = 0;
-    p.m = bp.m;
-    p.bluestein = true;
-    p.lanes = bp.lanes;
-    const int workers = (bp.m + 7) / 8 < 1024 / bp.lanes ? (bp.m + 7) / 8 : 1024 / bp.lanes;
-    p.block = dim3(bp.lanes, workers, 1);
-    p.smem = (size_t)bluestein_smem(n, bp.m, bp.lanes);
-  } else if (is_pow2(n) && n >= 4 && n <= 256) {
-    p.N = n;
-    const int workers = fftc::workers_for(n);
-    const int groups = workers >= 8 ? 1 : 8 / workers;
-    p.block = dim3(kLanes, workers, groups);
-    p.smem = two_pass_smem(n, kLanes, groups);
-  } else if (two_pass_smem(n, kLanes, 1) <= kMaxSmem) {
-    p.N = 0;
-    int workers = n >= 8 ? 8 : (n >= 4 ? 4 : 1);
-    if (mixed_radix_enabled()) {
-      p.rp = make_rt_plan(n);
-      // one output per worker-iteration: ~8 outputs per worker and pass, up to a full 1024-thread CTA
-      if (n > 64) workers = (n + 7) / 8 < 32 ? (n + 7) / 8 : 32;
-    }
-    const int groups = n <= 32 ? (8 / workers > 0 ? 8 / workers : 1) : 1;
-    p.block = dim3(kLanes, workers, groups);
-    p.smem = two_pass_smem(n, kLanes, groups);
-  } else {
-    // 448..1024 (longer lengths are rejected by check_fft_shapes): 8 channels per CTA, ~8 outputs per worker and
-    // pass, up to a full 1024-thread CTA
-    p.N = 0;
-    p.lanes = kNarrowLanes;
-    if (mixed_radix_enabled()) p.rp = make_rt_plan(n);
-    const int workers = (n + 7) / 8 < 1024 / kNarrowLanes ? (n + 7) / 8 : 1024 / kNarrowLanes;
-    p.block = dim3(kNarrowLanes, workers, 1);
-    p.smem = two_pass_smem(n, kNarrowLanes, 1);
-  }
-  return p;
-}
-
+// Launch plans of the two passes: fft_core.cuh (make_plan, make_plane_plans).
 template <typename K>
 int set_smem(K kernel, size_t bytes) {
   if (bytes > 48 * 1024) FFCB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
@@ -524,7 +436,7 @@ int rfft2(const ffcb_tensor* in, const ffcb_tensor* spec, void* ws, size_t ws_by
   const int C = in->C;
   const float scale = (float)(1.0 / sqrt((double)in->H * (double)in->W));
   {
-    LaunchPlan p = make_plan(in->W);
+    const LaunchPlan p = make_plane_plans(in->H, in->W).rows;
     const int pairs = in->B * ((in->H + 1) / 2);
     dim3 grid((pairs + p.block.z - 1) / p.block.z, (C + p.lanes - 1) / p.lanes);
     FFCB_DISPATCH_N(p, {
@@ -534,7 +446,7 @@ int rfft2(const ffcb_tensor* in, const ffcb_tensor* spec, void* ws, size_t ws_by
     FFCB_LAUNCH_CHECK("rfft_rows_kernel");
   }
   {
-    LaunchPlan p = make_plan(in->H);
+    const LaunchPlan p = make_plane_plans(in->H, in->W).cols;
     const int cols = in->B * spec->W;
     dim3 grid((cols + p.block.z - 1) / p.block.z, (C + p.lanes - 1) / p.lanes);
     FFCB_DISPATCH_N(p, {
@@ -577,7 +489,7 @@ int irfft2(const ffcb_tensor* spec, const ffcb_tensor* residual, const ffcb_tens
   const int C = out->C;
   const float scale = (float)(1.0 / sqrt((double)out->H * (double)out->W));
   {
-    LaunchPlan p = make_plan(out->H);
+    const LaunchPlan p = make_plane_plans(out->H, out->W).cols;
     const int cols = out->B * spec->W;
     dim3 grid((cols + p.block.z - 1) / p.block.z, (C + p.lanes - 1) / p.lanes);
     FFCB_DISPATCH_N(p, {
@@ -587,7 +499,7 @@ int irfft2(const ffcb_tensor* spec, const ffcb_tensor* residual, const ffcb_tens
     FFCB_LAUNCH_CHECK("fft_cols_inv_kernel");
   }
   {
-    LaunchPlan p = make_plan(out->W);
+    const LaunchPlan p = make_plane_plans(out->H, out->W).rows;
     const int pairs = out->B * ((out->H + 1) / 2);
     dim3 grid((pairs + p.block.z - 1) / p.block.z, (C + p.lanes - 1) / p.lanes);
     FFCB_DISPATCH_N(p, {

@@ -5,6 +5,8 @@
 // Data layout: data[point * LS + lane], LS = lane stride (32 on the device: lane == channel).
 #pragma once
 #include <math.h>
+#include <stddef.h>
+#include <stdlib.h>
 #include <vector_functions.h>
 #include <vector_types.h>
 
@@ -293,6 +295,101 @@ inline BluesteinPlan make_bluestein_plan(int n) {
   if (kBluesteinCostFactor * b.cost < (float)b.direct) { b.m = m; b.lanes = lanes; }
   return b;
 }
+
+// ---------------------------------------------------------------------------------------------
+// Launch plan of one axis of the two-pass kernels (fft.cu), host only; tests/host_emul/fft_plan_emul.cpp prints it.
+constexpr int kLanes = 32;        // channels per CTA of every length whose buffers fit
+constexpr int kNarrowLanes = 8;   // channels per CTA of lengths 448..1024, and of Bluestein lengths up to n = 512
+
+struct LaunchPlan {
+  int N;       // template length (0 = runtime length)
+  int n;       // runtime length
+  int m;       // Bluestein convolution length: 512, 1024 or 2048 (n otherwise)
+  bool bluestein;
+  int lanes;   // channels per CTA: kLanes, or kNarrowLanes (N == 0 only); Bluestein: bluestein_lanes
+  dim3 block;  // (lanes, workers, groups)
+  size_t smem;
+  RtPlan rp;   // N == 0 without Bluestein: runtime radix plan (np < 0: direct DFT)
+};
+
+// Lengths without a compile-time plan: runtime mixed-radix Stockham (FFCB_FFT_MIXED_RADIX=0 selects the O(n^2)
+// direct DFT they ran in the first revision — same results to round-off, kept as the cross-check; it turns Bluestein
+// off too).
+inline bool mixed_radix_enabled() {
+  const char* e = getenv("FFCB_FFT_MIXED_RADIX");
+  return e ? atoi(e) != 0 : true;
+}
+
+// Lengths with a large prime factor: Bluestein when the planner prices it below the runtime plan
+// (FFCB_FFT_BLUESTEIN=0 restores the runtime plans, kept as the cross-check).
+inline bool bluestein_enabled() {
+  const char* e = getenv("FFCB_FFT_BLUESTEIN");
+  return e ? atoi(e) != 0 : true;
+}
+
+inline bool is_pow2(int v) { return v > 0 && (v & (v - 1)) == 0; }
+
+inline size_t two_pass_smem(int n, int lanes, int groups) {
+  return sizeof(float2) * ((size_t)n + (size_t)groups * 2 * n * lanes);
+}
+
+inline LaunchPlan make_plan(int n) {
+  LaunchPlan p;
+  p.n = n;
+  p.m = n;
+  p.bluestein = false;
+  p.lanes = kLanes;
+  p.rp.np = -1;
+  for (int i = 0; i < kMaxRtPasses; ++i) p.rp.radix[i] = 1;
+  BluesteinPlan bp;
+  bp.m = 0;
+  if (!(is_pow2(n) && n >= 4 && n <= 256) && mixed_radix_enabled() && bluestein_enabled())
+    bp = make_bluestein_plan(n);
+  if (bp.m > 0) {
+    // Bluestein: one group of 8 (m = 512, 1024) or 4 (m = 2048) channels, m / 8 workers: one radix-8 butterfly per
+    // worker and pass, up to a full 1024-thread CTA (bluestein_lanes)
+    p.N = 0;
+    p.m = bp.m;
+    p.bluestein = true;
+    p.lanes = bp.lanes;
+    const int workers = (bp.m + 7) / 8 < 1024 / bp.lanes ? (bp.m + 7) / 8 : 1024 / bp.lanes;
+    p.block = dim3(bp.lanes, workers, 1);
+    p.smem = (size_t)bluestein_smem(n, bp.m, bp.lanes);
+  } else if (is_pow2(n) && n >= 4 && n <= 256) {
+    p.N = n;
+    const int workers = workers_for(n);
+    const int groups = workers >= 8 ? 1 : 8 / workers;
+    p.block = dim3(kLanes, workers, groups);
+    p.smem = two_pass_smem(n, kLanes, groups);
+  } else if (two_pass_smem(n, kLanes, 1) <= (size_t)kBluesteinSmemLimit) {
+    p.N = 0;
+    int workers = n >= 8 ? 8 : (n >= 4 ? 4 : 1);
+    if (mixed_radix_enabled()) {
+      p.rp = make_rt_plan(n);
+      // one output per worker-iteration: ~8 outputs per worker and pass, up to a full 1024-thread CTA
+      if (n > 64) workers = (n + 7) / 8 < 32 ? (n + 7) / 8 : 32;
+    }
+    const int groups = n <= 32 ? (8 / workers > 0 ? 8 / workers : 1) : 1;
+    p.block = dim3(kLanes, workers, groups);
+    p.smem = two_pass_smem(n, kLanes, groups);
+  } else {
+    // 448..1024 (longer lengths are rejected by check_fft_shapes): 8 channels per CTA, ~8 outputs per worker and
+    // pass, up to a full 1024-thread CTA
+    p.N = 0;
+    p.lanes = kNarrowLanes;
+    if (mixed_radix_enabled()) p.rp = make_rt_plan(n);
+    const int workers = (n + 7) / 8 < 1024 / kNarrowLanes ? (n + 7) / 8 : 1024 / kNarrowLanes;
+    p.block = dim3(kNarrowLanes, workers, 1);
+    p.smem = two_pass_smem(n, kNarrowLanes, 1);
+  }
+  return p;
+}
+
+// The two passes of an H x W plane, in either direction: the row passes transform along W, the column passes along H.
+struct PlanePlans {
+  LaunchPlan rows, cols;
+};
+inline PlanePlans make_plane_plans(int H, int W) { return PlanePlans{make_plan(W), make_plan(H)}; }
 
 // c[j] = exp(-+ i pi j^2 / n).  The phase is reduced exactly in integers (j^2 mod 2n) first: j^2 / n in float loses
 // it at n ~ 1000.

@@ -65,7 +65,8 @@ def ffc_generator(x: torch.Tensor, state: List[torch.Tensor], spec: str) -> torc
     g = _shell(state, spec)
     xc = x.contiguous()
     if not E.generator_supported(g, xc):
-        raise RuntimeError("lama_b200::ffc_generator: input shape / model outside the native path")
+        raise RuntimeError(f"lama_b200::ffc_generator: {xc.shape[-2]}x{xc.shape[-1]} input / model outside the native "
+                           f"path")
     with torch.no_grad():
         return E.run_module(g, "generator", (xc,))[0]
 

@@ -33,7 +33,7 @@ class GeneratorPipeline:
         hp, wp = (-(-height // pad_mod) * pad_mod, -(-width // pad_mod) * pad_mod) if u8 else (height, width)
         probe = torch.empty(batch, cin, hp, wp, device=dev)
         if not E.generator_supported(generator, probe):
-            raise ValueError("generator / shape is outside the native path")
+            raise ValueError(f"generator / {hp}x{wp} input is outside the native path")
         del probe
         if u8:
             metas = (torch.empty(batch, height, width, 3, dtype=torch.uint8, device="meta"),
