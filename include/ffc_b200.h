@@ -38,7 +38,8 @@
 extern "C" {
 #endif
 
-#define FFCB_VERSION 113 /* 0.1.3: ffcb_refine_l1_grad (0.1.2: ffcb_add, ffcb_head_bwd7; 0.1.1: ffcb_tensor gained cg / tile / sg) */
+#define FFCB_VERSION 114 /* 0.1.4: ffcb_relu_mask_pack, ffcb_relu_bwd_bits (0.1.3: ffcb_refine_l1_grad; 0.1.2: ffcb_add,
+                            ffcb_head_bwd7; 0.1.1: ffcb_tensor gained cg / tile / sg) */
 
 enum {
   FFCB_OK = 0,
@@ -254,6 +255,21 @@ int ffcb_fill_reflect_border(const ffcb_tensor* t, ffcb_stream_t stream);
 int ffcb_relu_bwd(const ffcb_tensor* dy, const ffcb_tensor* y, const ffcb_tensor* out, ffcb_stream_t stream);
 int ffcb_fold_reflect_border(const ffcb_tensor* gpad, const ffcb_tensor* add0, int add0_c0, const ffcb_tensor* add1,
                              int add1_c0, const ffcb_tensor* out, ffcb_stream_t stream);
+
+/*
+ * ReLU masks kept as bits (ffc.py:101, 133, 253-254, 354: the nn.ReLU backwards of the FourierUnit, the
+ * SpectralTransform's conv1, FFC_BN_ACT and the up-sampling stages only test the forward activation for sign), so that
+ * a forward+backward program can release the activation itself after the forward:
+ *   ffcb_relu_mask_pack: bits[((b*H + y)*W + x)*nw + c/32] bit c%32 = [y(b,y,x,c) > 0], nw = ceil(C/32), over the
+ *                        interior of the view (B, H, W, C of `y`); the nw*32 - C unused high bits of a pixel's last word
+ *                        are 0.  The value compared is the one ffcb_relu_bwd reads (hi + lo for FFCB_BF16X2).
+ *   ffcb_relu_bwd_bits:  out = dy * bit — ffcb_relu_bwd with the mask of `y` packed by ffcb_relu_mask_pack (bits
+ *                        sized by out's B, H, W, C), bit-identical to it.
+ * Both take every view ffcb_relu_bwd takes: either storage format, rings, channel slices, channel-group planar and
+ * tile-blocked views.  bits: device memory of B*H*W*nw uint32, 4-byte aligned.
+ */
+int ffcb_relu_mask_pack(const ffcb_tensor* y, uint32_t* bits, ffcb_stream_t stream);
+int ffcb_relu_bwd_bits(const ffcb_tensor* dy, const uint32_t* bits, const ffcb_tensor* out, ffcb_stream_t stream);
 
 /*
  * Input gradients through the generator's rear (residual blocks -> ConcatTupleLayer -> up-sampling tail -> head,

@@ -17,7 +17,7 @@ ACT_NONE, ACT_RELU, ACT_SIGMOID, ACT_TANH = 0, 1, 2, 3
 BORDER_ZERO, BORDER_REFLECT = 0, 1
 MATH_FP32, MATH_BF16X3 = 0, 1
 MAX_KSEG = 64
-VERSION = 113
+VERSION = 114
 
 
 class Tensor(C.Structure):
@@ -64,6 +64,8 @@ SIGNATURES = {
     "ffcb_nhwc_to_nchw": (C.c_int, [_PT, C.c_void_p, C.c_void_p]),
     "ffcb_fill_reflect_border": (C.c_int, [_PT, C.c_void_p]),
     "ffcb_relu_bwd": (C.c_int, [_PT, _PT, _PT, C.c_void_p]),
+    "ffcb_relu_mask_pack": (C.c_int, [_PT, C.c_void_p, C.c_void_p]),
+    "ffcb_relu_bwd_bits": (C.c_int, [_PT, C.c_void_p, _PT, C.c_void_p]),
     "ffcb_fold_reflect_border": (C.c_int, [_PT, _PT, C.c_int, _PT, C.c_int, _PT, C.c_void_p]),
     "ffcb_add": (C.c_int, [_PT, _PT, _PT, C.c_void_p]),
     "ffcb_head_bwd7": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,

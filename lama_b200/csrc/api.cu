@@ -80,6 +80,8 @@ int stem_pack_u8(const uint8_t*, const uint8_t*, int, int, int, const ffcb_tenso
 int head_gather7_blend_u8(const ffcb_tensor*, const float*, int, const uint8_t*, const uint8_t*, int, int, uint8_t*,
                           cudaStream_t);
 int relu_bwd(const ffcb_tensor*, const ffcb_tensor*, const ffcb_tensor*, cudaStream_t);
+int relu_mask_pack(const ffcb_tensor*, uint32_t*, cudaStream_t);
+int relu_bwd_bits(const ffcb_tensor*, const uint32_t*, const ffcb_tensor*, cudaStream_t);
 int fold_reflect_border(const ffcb_tensor*, const ffcb_tensor*, int, const ffcb_tensor*, int, const ffcb_tensor*,
                         cudaStream_t);
 int add(const ffcb_tensor*, const ffcb_tensor*, const ffcb_tensor*, cudaStream_t);
@@ -210,6 +212,14 @@ int ffcb_fill_reflect_border(const ffcb_tensor* t, ffcb_stream_t stream) {
 
 int ffcb_relu_bwd(const ffcb_tensor* dy, const ffcb_tensor* y, const ffcb_tensor* out, ffcb_stream_t stream) {
   return relu_bwd(dy, y, out, (cudaStream_t)stream);
+}
+
+int ffcb_relu_mask_pack(const ffcb_tensor* y, uint32_t* bits, ffcb_stream_t stream) {
+  return relu_mask_pack(y, bits, (cudaStream_t)stream);
+}
+
+int ffcb_relu_bwd_bits(const ffcb_tensor* dy, const uint32_t* bits, const ffcb_tensor* out, ffcb_stream_t stream) {
+  return relu_bwd_bits(dy, bits, out, (cudaStream_t)stream);
 }
 
 int ffcb_fold_reflect_border(const ffcb_tensor* gpad, const ffcb_tensor* add0, int add0_c0, const ffcb_tensor* add1,

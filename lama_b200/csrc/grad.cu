@@ -10,6 +10,8 @@
 //   ffcb_relu_bwd             dx = dy * [y > 0]                      (y = the forward activation, ffc.py:101,133,253-254)
 //   ffcb_fold_reflect_border  adjoint of ReflectionPad(1): the gradient w.r.t. the padded plane folded back onto the
 //                             interior (+ up to two addends: the 1x1 branch's gradient, the residual path's gradient)
+//   ffcb_relu_mask_pack       bits = [y > 0], one bit per element, so that the refinement step program can drop the
+//   ffcb_relu_bwd_bits        full-width forward activations after the forward; dx = dy * bit is ffcb_relu_bwd
 // and, for the generator's rear (residual blocks + up-sampling tail + head, lama_b200/engine.py:
 // build_rear_grad_program):
 //   ffcb_add                  out = a + b over the padded extent (the block identity X + Y2, ffc.py:288, with Y2 kept)
@@ -45,6 +47,66 @@ __global__ void relu_bwd_kernel(View dy, View y, View out) {
     const float4 g = load4g(dy, b, yy, x, 4 * q), a = load4g(y, b, yy, x, 4 * q);
     store4g(out, b, yy, x, 4 * q,
             make_float4(a.x > 0.f ? g.x : 0.f, a.y > 0.f ? g.y : 0.f, a.z > 0.f ? g.z : 0.f, a.w > 0.f ? g.w : 0.f));
+  }
+}
+
+// ---- bit-packed ReLU masks: word ((b*H + y)*W + x)*nw + c/32 of a view holds bit c%32 = [y(b,y,x,c) > 0] ----------
+// The comparison reads the value exactly as relu_bwd_kernel does (load1 / load4 decode split bf16 as hi + lo in the
+// same float addition), so relu_bwd_bits_kernel with these words writes what relu_bwd_kernel writes with the values.
+
+// channels-last views: one warp per (pixel, 32-channel word), lane l tests channel 32w + l and __ballot_sync builds
+// the word (a warp reads 32 adjacent channels: 128 contiguous bytes per fp32 plane, 64 per bf16 plane)
+__global__ void relu_mask_pack_cl_kernel(View y, uint32_t* __restrict__ bits, int nw) {
+  const long long total = (long long)y.B * y.H * y.W * nw;
+  const int lane = threadIdx.x & 31;
+  const long long nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
+  // every lane of a warp has the same i, so the whole warp takes part in each ballot
+  for (long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < total; i += nwarps) {
+    const int w = (int)(i % nw);
+    const long long p = i / nw;
+    const int x = (int)(p % y.W), yy = (int)((p / y.W) % y.H), b = (int)(p / ((long long)y.W * y.H));
+    const int c = 32 * w + lane;
+    const bool on = c < y.C && load1(y, pix_off(y, b, yy, x) + c) > 0.f;
+    const unsigned word = __ballot_sync(0xffffffffu, on);
+    if (lane == 0) bits[i] = word;
+  }
+}
+
+// channel-group planar / tile-blocked views: one thread per (pixel, word), pixels fastest so that neighbouring threads
+// read neighbouring pixels of one group plane; 4-channel loads never straddle a group (C % 4 == 0, cg in {4, 8})
+__global__ void relu_mask_pack_cg_kernel(View y, uint32_t* __restrict__ bits, int nw) {
+  const long long npix = (long long)y.B * y.H * y.W;
+  const long long total = npix * nw;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int w = (int)(i / npix);
+    const long long p = i % npix;
+    const int x = (int)(p % y.W), yy = (int)((p / y.W) % y.H), b = (int)(p / ((long long)y.W * y.H));
+    unsigned word = 0;
+    for (int k = 0; k < 32 && 32 * w + k < y.C; k += 4) {
+      const float4 a = load4g(y, b, yy, x, 32 * w + k);
+      word |= ((unsigned)(a.x > 0.f) | (unsigned)(a.y > 0.f) << 1 | (unsigned)(a.z > 0.f) << 2 |
+               (unsigned)(a.w > 0.f) << 3) << k;
+    }
+    bits[p * nw + w] = word;
+  }
+}
+
+// relu_bwd_kernel with the mask read from the packed words: the same loop order, loads and stores
+__global__ void relu_bwd_bits_kernel(View dy, const uint32_t* __restrict__ bits, int nw, View out) {
+  const int c4 = out.C / 4;
+  const long long total = (long long)out.B * out.H * out.W * c4;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int q = out.cg ? (int)(i / ((long long)out.B * out.H * out.W)) : (int)(i % c4);
+    const long long p = out.cg ? i % ((long long)out.B * out.H * out.W) : i / c4;
+    const int x = (int)(p % out.W);
+    const int yy = (int)((p / out.W) % out.H);
+    const int b = (int)(p / ((long long)out.W * out.H));
+    const float4 g = load4g(dy, b, yy, x, 4 * q);
+    const unsigned m = __ldg(bits + p * nw + (q >> 3)) >> (4 * (q & 7));     // channels 4q .. 4q+3
+    store4g(out, b, yy, x, 4 * q,
+            make_float4((m & 1u) ? g.x : 0.f, (m & 2u) ? g.y : 0.f, (m & 4u) ? g.z : 0.f, (m & 8u) ? g.w : 0.f));
   }
 }
 
@@ -215,6 +277,39 @@ int relu_bwd(const ffcb_tensor* dy, const ffcb_tensor* y, const ffcb_tensor* out
   if (total == 0) return FFCB_OK;
   relu_bwd_kernel<<<grid_for(total), 256, 0, stream>>>(make_view(*dy), make_view(*y), make_view(*out));
   FFCB_LAUNCH_CHECK("relu_bwd_kernel");
+  return FFCB_OK;
+}
+
+int relu_mask_pack(const ffcb_tensor* y, uint32_t* bits, cudaStream_t stream) {
+  int rc;
+  if ((rc = check_tensor(y, "relu_mask_pack.y", true))) return rc;
+  const long long npix = (long long)y->B * y->H * y->W;
+  if (npix * y->C == 0) return FFCB_OK;
+  FFCB_REQUIRE(bits != nullptr && ((uintptr_t)bits % 4) == 0, "relu_mask_pack: bits must be a 4-byte aligned pointer");
+  const int nw = (y->C + 31) / 32;
+  const View v = make_view(*y);
+  if (v.cg) {
+    relu_mask_pack_cg_kernel<<<grid_for(npix * nw), 256, 0, stream>>>(v, bits, nw);
+    FFCB_LAUNCH_CHECK("relu_mask_pack_cg_kernel");
+  } else {
+    relu_mask_pack_cl_kernel<<<grid_for(npix * nw * 32), 256, 0, stream>>>(v, bits, nw);
+    FFCB_LAUNCH_CHECK("relu_mask_pack_cl_kernel");
+  }
+  return FFCB_OK;
+}
+
+int relu_bwd_bits(const ffcb_tensor* dy, const uint32_t* bits, const ffcb_tensor* out, cudaStream_t stream) {
+  int rc;
+  if ((rc = check_tensor(dy, "relu_bwd_bits.dy", true)) || (rc = check_tensor(out, "relu_bwd_bits.out", true)))
+    return rc;
+  FFCB_REQUIRE(dy->B == out->B && dy->H == out->H && dy->W == out->W && dy->C == out->C,
+               "relu_bwd_bits: shapes differ");
+  const long long total = (long long)out->B * out->H * out->W * (out->C / 4);
+  if (total == 0) return FFCB_OK;
+  FFCB_REQUIRE(bits != nullptr && ((uintptr_t)bits % 4) == 0, "relu_bwd_bits: bits must be a 4-byte aligned pointer");
+  relu_bwd_bits_kernel<<<grid_for(total), 256, 0, stream>>>(make_view(*dy), bits, (out->C + 31) / 32,
+                                                            make_view(*out));
+  FFCB_LAUNCH_CHECK("relu_bwd_bits_kernel");
   return FFCB_OK;
 }
 

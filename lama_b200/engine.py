@@ -50,6 +50,7 @@ class Buf:
     reflect_border: int = 0
     cg: int = 0        # > 0: channel-group planar storage [C/cg][B][H][W][cg] (FourierUnit chain, include/ffc_b200.h)
     tile: int = 0      # 128 (with cg == 8, split bf16): tile-blocked [pixel block of 128][C/8][128][8] — wgmma operand tiles
+    bits: int = 0      # 1: a ReLU mask, one bit per element — uint32 words [B][H][W][ceil(C/32)] (lama_b200.relu_bits)
 
 
 @dataclass
@@ -98,7 +99,7 @@ class Ext:
     name: str
 
 
-OP_TYPES: List[type] = []       # every op record type (tests check that each one is fully declared)
+OP_TYPES: List[type] = []       # every op record type of the default programs (tests check that each one is fully declared)
 
 # What an op does to the reflected ring of a buffer it writes:
 STALE = "stale"          # the interior changes, the ring does not: insert_border_ops refreshes it before a ring read
@@ -111,15 +112,16 @@ class Op:
     (``reads`` / ``writes``; a field may hold a view, None, or a list of views or of (view, int) pairs), its ring
     effect on the buffers it writes and the reads that need a valid ring (``ring_in``), its FFT workspace and scratch,
     and ``bind(ex)``: its one C-ABI call on executor ``ex`` as (call name, library function, argument list without the
-    trailing stream), or None."""
+    trailing stream), or None.  A subclass joins ``OP_TYPES``, or the list given as its ``registry`` class argument
+    (the op types of an opt-in program variant defined in another module)."""
     reads: Tuple[str, ...]          # every op type sets both
     writes: Tuple[str, ...]
     ring_in: Tuple[str, ...] = ()
     ring = STALE
 
-    def __init_subclass__(cls, **kw):
+    def __init_subclass__(cls, registry: Optional[List[type]] = None, **kw):
         super().__init_subclass__(**kw)
-        OP_TYPES.append(cls)
+        (OP_TYPES if registry is None else registry).append(cls)
 
     def _tvs(self, names) -> List[TV]:
         flat = [x for v in (getattr(self, n) for n in names) for x in (v if isinstance(v, list) else [v])]
@@ -1062,6 +1064,9 @@ def build_module_program(module, kind: str, shapes: Sequence[Optional[Tuple[int,
     elif kind.startswith("generator_refine:"):          # "generator_refine:<H0>x<W0>" (crop of the prediction)
         h0, w0 = (int(v) for v in kind.split(":")[1].split("x"))
         build_refine_program(prog, module, shapes[0], shapes[1], (h0, w0))
+    elif kind.startswith("generator_refine_bits:"):     # the same step, ReLU masks kept as bits (relu_masks="bits")
+        h0, w0 = (int(v) for v in kind.split(":")[1].split("x"))
+        build_refine_program(prog, module, shapes[0], shapes[1], (h0, w0), relu_masks="bits")
     elif kind.startswith("generator_u8"):            # "generator_u8:<pad modulo>", shapes = (img, mask)
         mod = int(kind.split(":")[1]) if ":" in kind else 8
         b, h0, w0, _ = shapes[0]
@@ -1283,14 +1288,19 @@ def refine_supported(gen, shape_l, shape_g, crop: Tuple[int, int]) -> bool:
     return lay[5].out_channels == 3 and 3 <= crop[0] <= H and 3 <= crop[1] <= W
 
 
-def build_refine_program(prog: Program, gen, sl: Tuple[int, ...], sg: Tuple[int, ...], crop: Tuple[int, int]):
+def build_refine_program(prog: Program, gen, sl: Tuple[int, ...], sg: Tuple[int, ...], crop: Tuple[int, int],
+                         relu_masks: str = "values"):
     """One Adam step of the refinement loop (evaluation/refinement.py:137-167) without the optimiser:
     rear forward | SplitOp | RefineLossOp | rear backward.
     inputs  x0, x1 (z1, z2), and the per-scale constants image (B,3,H,W), mask (B,1,H,W) in {0,1}, ref (B,3,H0/2,W0/2),
             md (B,1,H0/2,W0/2) (the eroded down-scaled mask), inv (B,2) (1 / n_out, 1 / n_down, 0 for an empty term);
     outputs y0 (pred), dy0 (dL/dpred, written by RefineLossOp and read by the head adjoint), loss (B,2), dx0, dx1.
-    ``run(part=0)`` alone is the forward-only rear (the last forward of a scale, and the lowest scale)."""
+    ``run(part=0)`` alone is the forward-only rear (the last forward of a scale, and the lowest scale).
+    ``relu_masks="bits"``: the backward's ReLU masks of forward activations are kept as bits
+    (``relu_bits.pack_relu_masks``): the same results in less than half the storage at large planes."""
     from .refine import gaussian_kernel1d
+    if relu_masks not in ("values", "bits"):
+        raise ValueError(f"relu_masks must be 'values' or 'bits', not {relu_masks!r}")
     h0, w0 = crop
     fwd = emit_rear_forward(prog, gen, sl, sg)
     b, n, H, W = prog.outputs["y0"]
@@ -1301,6 +1311,9 @@ def build_refine_program(prog: Program, gen, sl: Tuple[int, ...], sg: Tuple[int,
     prog.ops.append(RefineLossOp("y0", "image", "mask", "ref", "md", "inv", h0, w0, gaussian_kernel1d(5, 1.0),
                                  "dy0", "loss", b * n * (h0 // 2) * (w0 // 2)))
     emit_rear_backward(prog, gen, fwd, "dy0")
+    if relu_masks == "bits":
+        from .relu_bits import pack_relu_masks
+        pack_relu_masks(prog)
 
 
 def tc_compatible(prog: Program) -> bool:
@@ -1358,11 +1371,14 @@ def op_scratch_bytes(op) -> int:
 
 def storage_key(b: Buf) -> tuple:
     """Buffers with equal keys have byte-identical storage (dtype, shape, ring, layout)."""
-    return (b.fmt, b.B, b.H, b.W, b.C, b.pad, b.reflect_border, b.cg, b.tile)
+    return (b.fmt, b.B, b.H, b.W, b.C, b.pad, b.reflect_border, b.cg, b.tile, b.bits)
 
 
 def storage_shape(b: Buf) -> Tuple[int, ...]:
-    """Shape of a buffer's storage tensor: float32, or bfloat16 with a leading 2 (hi / lo halves) for split bf16."""
+    """Shape of a buffer's storage tensor: float32, or bfloat16 with a leading 2 (hi / lo halves) for split bf16, or
+    int32 words of 32 mask bits for a bit mask."""
+    if b.bits:
+        return (b.B, b.H, b.W, -(-b.C // 32))
     if b.tile:
         return (-(-(b.B * b.H * b.W) // 128), b.C // 8, 128, 8)      # zero-initialised: the tail block stays finite
     if b.cg:
@@ -1379,7 +1395,7 @@ def program_storage_bytes(prog: Program) -> int:
     for b in prog.bufs:
         if slots[b.name] not in seen:
             seen.add(slots[b.name])
-            total += 4 * math.prod(storage_shape(b))           # float32, or two bfloat16 halves
+            total += 4 * math.prod(storage_shape(b))           # float32, two bfloat16 halves, or int32 mask words
     for name, shape in prog.outputs.items():
         total += math.prod(shape) * (1 if prog.dtypes.get(name, torch.float32) == torch.uint8 else 4)
     return total + max(prog.fft_workspace_bytes(), 16) + sum(op.scratch_bytes() for op in prog.ops)
@@ -1438,7 +1454,9 @@ class CudaExecutor:
                 self.storage[b.name] = slot_tensor[si]
                 continue
             shape = storage_shape(b)
-            if b.fmt == L.F32:
+            if b.bits:
+                slot_tensor[si] = torch.zeros(shape, dtype=torch.int32, device=device)
+            elif b.fmt == L.F32:
                 slot_tensor[si] = torch.empty(shape, dtype=torch.float32, device=device)
             else:
                 slot_tensor[si] = torch.zeros((2,) + shape, dtype=torch.bfloat16, device=device)

@@ -292,13 +292,20 @@ def build_parser() -> argparse.ArgumentParser:
     ap.add_argument("--min-side", type=int, default=512, help="refinement: smallest side of the lowest scale")
     ap.add_argument("--max-scales", type=int, default=3, help="refinement: most pyramid scales")
     ap.add_argument("--px-budget", type=int, default=1800000, help="refinement: larger images are resized to this")
+    ap.add_argument("--relu-masks", choices=("values", "bits"), default=None,
+                    help="refinement: keep the backward's ReLU masks as the forward activations (values, the default) "
+                         "or as bits, which needs about half the memory at large scales (same results), e.g. to "
+                         "refine 12-24 megapixel photos at full size with a raised --px-budget")
     return ap
 
 
 def refiner_kwargs(a: argparse.Namespace) -> Dict:
-    """Command-line arguments -> lama_b200.refine.BatchedRefiner keyword arguments."""
-    return dict(max_batch=a.batch, modulo=a.pad_mod, n_iters=a.n_iters, lr=a.lr, min_side=a.min_side,
-                max_scales=a.max_scales, px_budget=a.px_budget)
+    """Command-line arguments -> lama_b200.refine.BatchedRefiner keyword arguments (``relu_masks`` only when given)."""
+    kw = dict(max_batch=a.batch, modulo=a.pad_mod, n_iters=a.n_iters, lr=a.lr, min_side=a.min_side,
+              max_scales=a.max_scales, px_budget=a.px_budget)
+    if a.relu_masks is not None:
+        kw["relu_masks"] = a.relu_masks
+    return kw
 
 
 def main(argv=None):

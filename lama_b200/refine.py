@@ -226,10 +226,11 @@ class _StepLane:
     (rear forward, loss gradient, rear backward, Adam), captured on first use and replayed for every later batch and
     scale of the same shape."""
 
-    def __init__(self, gen, sl, sg, crop, lr: float, device, graphs: bool = True):
+    def __init__(self, gen, sl, sg, crop, lr: float, device, graphs: bool = True, kind: Optional[str] = None):
         from . import engine as E
+        kind = kind if kind is not None else f"generator_refine:{crop[0]}x{crop[1]}"
         with torch.no_grad():
-            prog = E.build_module_program(gen, f"generator_refine:{crop[0]}x{crop[1]}", (sl, sg), E.default_math())
+            prog = E.build_module_program(gen, kind, (sl, sg), E.default_math())
         self.ex = E.CudaExecutor(prog, device)
         self.inputs = {k: torch.zeros(v, dtype=torch.float32, device=device) for k, v in prog.inputs.items()}
         self.z = [self.inputs["x0"].requires_grad_(True), self.inputs["x1"].requires_grad_(True)]
@@ -301,11 +302,24 @@ class BatchedRefiner:
     (default: 70 % of the free device memory when the group starts).  A group is cut into balanced batches, and the
     programs of one batch size are released before those of another are built, so no more than one batch's programs are
     alive at a time.  An image whose programs alone exceed the budget still runs, at batch 1; if the device cannot hold
-    them, the allocation error propagates to the caller."""
+    them, the allocation error propagates to the caller.
+
+    ``relu_masks="bits"`` runs the step programs of kind ``generator_refine_bits``: the ReLU masks the backward reads
+    are kept as bits instead of the forward activations themselves (``lama_b200.relu_bits``), which cuts a step
+    program's storage by about 53 % at large scales, so that 12- and 24-megapixel photos refine at full size on one
+    80 GB GPU.  The results are bit-identical to ``"values"``.  This large-photo setting also keeps one scale's program
+    alive at a time (a scale's lane releases the previous one; the batch plan still counts every scale) and releases the
+    front's (stem and down-sampling) cached stage programs after each scale's front pass, which at 24 MP would otherwise
+    hold about 34 GB next to the step programs.  Later batches of the same size build and capture them again."""
+
+    relu_masks = "values"
 
     def __init__(self, generator, max_batch: int = 8, *, modulo: int = 8, n_iters: int = 15, lr: float = 0.002,
                  min_side: int = 512, max_scales: int = 3, px_budget: int = 1800000,
-                 mem_budget: Optional[int] = None):
+                 mem_budget: Optional[int] = None, relu_masks: str = "values"):
+        if relu_masks not in ("values", "bits"):
+            raise ValueError(f"relu_masks must be 'values' or 'bits', not {relu_masks!r}")
+        self.relu_masks = relu_masks
         self.generator = generator.eval()
         self.device = next(generator.parameters()).device
         if self.device.type != "cuda":
@@ -369,10 +383,12 @@ class BatchedRefiner:
         shapes = self.scale_shapes(h, w)
         return bool(shapes) and all(E.refine_supported(self.generator, sl, sg, crop) for sl, sg, crop in shapes)
 
-    @staticmethod
-    def program_kind(scale: int, crop: Tuple[int, int]) -> str:
-        """The lowest scale (index 0) runs one forward; every other scale a step program."""
-        return "generator_rear" if scale == 0 else f"generator_refine:{crop[0]}x{crop[1]}"
+    def program_kind(self, scale: int, crop: Tuple[int, int]) -> str:
+        """The lowest scale (index 0) runs one forward; every other scale a step program (``relu_masks``: which)."""
+        if scale == 0:
+            return "generator_rear"
+        step = "generator_refine_bits" if self.relu_masks == "bits" else "generator_refine"
+        return f"{step}:{crop[0]}x{crop[1]}"
 
     def per_image_bytes(self, h: int, w: int) -> int:
         """Pooled device bytes of the one-image programs of every scale of an (h, w) input (a batch keeps all of them
@@ -389,13 +405,13 @@ class BatchedRefiner:
     def _make_lane(self, kind: str, sl, sg, crop):
         if kind == "generator_rear":
             return _ForwardLane(self.generator, sl, sg, self.device)
-        return _StepLane(self.generator, sl, sg, crop, self.kw["lr"], self.device, self._graphs)
+        return _StepLane(self.generator, sl, sg, crop, self.kw["lr"], self.device, self._graphs, kind)
 
     def _lane(self, b: int, scale: int, sl, sg, crop):
         """The lane of scale ``scale`` at batch size ``b``.  Lanes of another batch size are released first: only one
         batch's programs are alive at a time, which is what the batch plan budgets for."""
         key = (b, sl[1:], sg[1:], crop)
-        if any(k[0] != b for k in self._lanes):
+        if any(k[0] != b for k in self._lanes) or (self.relu_masks == "bits" and key not in self._lanes):
             self._lanes.clear()
             torch.cuda.empty_cache()
         lane = self._lanes.get(key)
@@ -419,6 +435,12 @@ class BatchedRefiner:
             mk = (mk >= 1e-8).to(mk.dtype)
             with torch.no_grad():
                 z1, z2 = self.front(torch.cat([im * (1 - mk), mk], dim=1))
+            if self.relu_masks == "bits":
+                # the front's cached stage programs hold full-resolution buffers (about 34 GB for a 24 MP scale); the
+                # large-photo setting releases them before the step program of the scale is built
+                from . import engine as E
+                for m in self.front.modules():
+                    E.invalidate(m)
             lane = self._lane(len(images), s, sl, sg, crop)
             h0, w0 = crop
             consts = dict(image=im, mask=mk)
