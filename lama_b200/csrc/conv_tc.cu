@@ -608,35 +608,48 @@ conv_tc_kernel(const __grid_constant__ TcParams p, const __grid_constant__ CUten
         }
       }
       const uint64_t pol = l2_policy(PO && p.hints ? 2 : 0);      // planar outputs: consumed by the next kernel
+      // Shift and addend of EB column groups are loaded before any of their stores: the stores may alias the addend
+      // (an in-place residual), so loads placed after them would each wait a full global-memory round trip.
+      constexpr int EB = (BN / 8) % 8 == 0 ? 8 : 4;
+      static_assert((BN / 8) % EB == 0, "whole batches of column groups");
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        // lane pairs swap half of their 8-column group: even lanes keep row r, odd lanes row r + 8
-        const float s0 = odd ? acc[4 * j] : acc[4 * j + 2], s1 = odd ? acc[4 * j + 1] : acc[4 * j + 3];
-        const float r0 = __shfl_xor_sync(0xffffffffu, s0, 1), r1 = __shfl_xor_sync(0xffffffffu, s1, 1);
-        float4 v = odd ? make_float4(r0, r1, acc[4 * j + 2], acc[4 * j + 3])
-                       : make_float4(acc[4 * j], acc[4 * j + 1], r0, r1);
-        const int n = n_tile * p.BN + 8 * j + cb;
-        if (!valid || n >= p.N) continue;
-        if (p.shift != nullptr) {
-          const float4 sh = __ldg(reinterpret_cast<const float4*>(p.shift + n));
+      for (int j0 = 0; j0 < BN / 8; j0 += EB) {
+        float4 shv[EB], adv[EB];
+#pragma unroll
+        for (int i = 0; i < EB; ++i) {
+          const int n = n_tile * p.BN + 8 * (j0 + i) + cb;
+          const bool ok = valid && n < p.N;
+          shv[i] = (ok && p.shift != nullptr) ? __ldg(reinterpret_cast<const float4*>(p.shift + n))
+                                               : make_float4(0.f, 0.f, 0.f, 0.f);
+          adv[i] = (ok && has_add) ? load4(p.addend, o_add + n) : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+#pragma unroll
+        for (int i = 0; i < EB; ++i) {
+          const int j = j0 + i;
+          // lane pairs swap half of their 8-column group: even lanes keep row r, odd lanes row r + 8
+          const float s0 = odd ? acc[4 * j] : acc[4 * j + 2], s1 = odd ? acc[4 * j + 1] : acc[4 * j + 3];
+          const float r0 = __shfl_xor_sync(0xffffffffu, s0, 1), r1 = __shfl_xor_sync(0xffffffffu, s1, 1);
+          float4 v = odd ? make_float4(r0, r1, acc[4 * j + 2], acc[4 * j + 3])
+                         : make_float4(acc[4 * j], acc[4 * j + 1], r0, r1);
+          const int n = n_tile * p.BN + 8 * j + cb;
+          if (!valid || n >= p.N) continue;
+          const float4 sh = shv[i], ad = adv[i];
           v.x += sh.x; v.y += sh.y; v.z += sh.z; v.w += sh.w;
-        }
-        float4 ad = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (has_add) ad = load4(p.addend, o_add + n);
-        if (!p.addend_post) { v.x += ad.x; v.y += ad.y; v.z += ad.z; v.w += ad.w; }
-        if (p.act == FFCB_ACT_RELU) {
-          v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
-        } else if (p.act != FFCB_ACT_NONE) {
-          v.x = slow_act(v.x, p.act); v.y = slow_act(v.y, p.act); v.z = slow_act(v.z, p.act); v.w = slow_act(v.w, p.act);
-        }
-        if (p.addend_post) { v.x += ad.x; v.y += ad.y; v.z += ad.z; v.w += ad.w; }
-        if constexpr (PO) {
-          st_hint_f4(reinterpret_cast<float*>(p.out.ptr) + o_out + chan_off(p.out, n), v, pol);
-        } else {
-          store4(p.out, o_out + n, v);
-          if (mir_dy) store4(p.out, o_out + mir_dy + n, v);
-          if (mir_dx) store4(p.out, o_out + mir_dx + n, v);
-          if (mir_dy && mir_dx) store4(p.out, o_out + mir_dy + mir_dx + n, v);
+          if (!p.addend_post) { v.x += ad.x; v.y += ad.y; v.z += ad.z; v.w += ad.w; }
+          if (p.act == FFCB_ACT_RELU) {
+            v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
+          } else if (p.act != FFCB_ACT_NONE) {
+            v.x = slow_act(v.x, p.act); v.y = slow_act(v.y, p.act); v.z = slow_act(v.z, p.act); v.w = slow_act(v.w, p.act);
+          }
+          if (p.addend_post) { v.x += ad.x; v.y += ad.y; v.z += ad.z; v.w += ad.w; }
+          if constexpr (PO) {
+            st_hint_f4(reinterpret_cast<float*>(p.out.ptr) + o_out + chan_off(p.out, n), v, pol);
+          } else {
+            store4(p.out, o_out + n, v);
+            if (mir_dy) store4(p.out, o_out + mir_dy + n, v);
+            if (mir_dx) store4(p.out, o_out + mir_dx + n, v);
+            if (mir_dy && mir_dx) store4(p.out, o_out + mir_dy + mir_dx + n, v);
+          }
         }
       }
     }
@@ -801,8 +814,8 @@ int conv_tc(const ffcb_conv_desc* d, cudaStream_t stream) {
   // column-halo mode (TcParams::seg_taps): spatial, stride 1, planes wider than 32 (the current tiling's TW >= 64),
   // and channels-last outputs; every segment reads a reflect-ring-padded channels-last source within one pixel
   // (coord_off >= 1); at least one complete 3x3 group.  Contractions with a tile-blocked segment (the global one:
-  // convl2g + st.conv2) keep the per-tap path: each of its one-tap groups would wait for an A buffer to turn over
-  // (DESIGN.md §9).
+  // convl2g + st.conv2) keep the per-tap path: on big-lama's 64-wide planes the column-halo mode measured 1-4 % slower
+  // for them, even with two tile-blocked K blocks per A buffer (DESIGN.md §9).
   bool halo = !flat && !rr && d->stride == 1 && W > 32 && d->out.cg == 0;
   int ngroups = 0;
   for (int i = 0; i < d->nseg && halo;) {
