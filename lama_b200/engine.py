@@ -577,42 +577,125 @@ def _generator_layout(gen):
         if not isinstance(mods[i], ConcatTupleLayer):
             return None
         i += 1
-        ups = []
-        while isinstance(mods[i], nn.ConvTranspose2d):
-            ct, bn, act = mods[i], mods[i + 1], mods[i + 2]
-            if not (ct.kernel_size == (3, 3) and ct.stride == (2, 2) and ct.padding == (1, 1)
-                    and ct.output_padding == (1, 1) and ct.groups == 1 and ct.dilation == (1, 1)
-                    and isinstance(bn, nn.BatchNorm2d) and bn_foldable(bn) and isinstance(act, nn.ReLU)
-                    and ct.in_channels % 4 == 0 and ct.out_channels % 4 == 0):
-                return None
-            ups.append((ct, bn)); i += 3
+        ups, i = _up_stages(mods, i)
+        if ups is None:
+            return None
         out_blk = None
         if isinstance(mods[i], FFCResnetBlock):          # out_ffc=True (ffc.py:356-358): an inline block at full resolution
             if not (mods[i].inline and mods[i].native_supported()):
                 return None
             out_blk = mods[i]; i += 1
-        if not (isinstance(mods[i], nn.ReflectionPad2d) and tuple(mods[i].padding) == (3, 3, 3, 3)):
-            return None
-        head = mods[i + 1]
-        if not (isinstance(head, nn.Conv2d) and head.kernel_size == (7, 7) and head.padding == (0, 0)
-                and head.stride == (1, 1) and head.groups == 1 and head.out_channels <= 4
-                and head.in_channels % 4 == 0):
-            return None
-        i += 2
-        out_act = L.ACT_NONE
-        if i < len(mods):
-            out_act = _act_code(mods[i])
-            if out_act is None:
-                return None
-            i += 1
-        if i != len(mods):
+        head, out_act = _head_stage(mods, i)
+        if head is None:
             return None
         return stem, downs, blocks, ups, out_blk, head, out_act
     except IndexError:
         return None
 
 
+def _up_stages(mods, i):
+    """ConvTranspose2d(k3, s2, p1, op1) + BN + ReLU stages from ``mods[i]`` on (ffc.py:350-354, pix2pixhd.py:424-429):
+    ([(ct, bn)], index after them), or (None, i) when one of them is off the native path."""
+    ups = []
+    while isinstance(mods[i], nn.ConvTranspose2d):
+        ct, bn, act = mods[i], mods[i + 1], mods[i + 2]
+        if not (ct.kernel_size == (3, 3) and ct.stride == (2, 2) and ct.padding == (1, 1)
+                and ct.output_padding == (1, 1) and ct.groups == 1 and ct.dilation == (1, 1)
+                and isinstance(bn, nn.BatchNorm2d) and bn_foldable(bn) and isinstance(act, nn.ReLU)
+                and ct.in_channels % 4 == 0 and ct.out_channels % 4 == 0):
+            return None, i
+        ups.append((ct, bn)); i += 3
+    return ups, i
+
+
+def _head_stage(mods, i):
+    """ReflectionPad2d(3) + Conv2d 7x7 [+ activation] ending ``mods`` at ``mods[i]`` (ffc.py:360-363,
+    pix2pixhd.py:430-433): (head conv, activation code), or (None, None)."""
+    if not (isinstance(mods[i], nn.ReflectionPad2d) and tuple(mods[i].padding) == (3, 3, 3, 3)):
+        return None, None
+    head = mods[i + 1]
+    if not (isinstance(head, nn.Conv2d) and head.kernel_size == (7, 7) and head.padding == (0, 0)
+            and head.stride == (1, 1) and head.groups == 1 and head.out_channels <= 4
+            and head.in_channels % 4 == 0):
+        return None, None
+    i += 2
+    out_act = L.ACT_NONE
+    if i < len(mods):
+        out_act = _act_code(mods[i])
+        if out_act is None:
+            return None, None
+        i += 1
+    return (head, out_act) if i == len(mods) else (None, None)
+
+
+def _affine_bn(bn) -> bool:
+    return isinstance(bn, nn.BatchNorm2d) and bn.affine and bn_foldable(bn)
+
+
+def _biased_conv(conv, k: int, stride: int, padding: int, padding_mode: str) -> bool:
+    return (type(conv) is nn.Conv2d and conv.kernel_size == (k, k) and conv.stride == (stride, stride)
+            and conv.padding == (padding, padding) and conv.dilation == (1, 1) and conv.groups == 1
+            and conv.padding_mode == padding_mode and conv.in_channels % 4 == 0 and conv.out_channels % 4 == 0)
+
+
+def _global_layout(gen):
+    """Parse the ``model`` of a LaMa-Regular generator (``lama_b200.pix2pixhd.GlobalGenerator``,
+    pix2pixhd.py:341-436) into (stem conv, stem bn, downs [(conv, bn)], blocks [(conv1, bn1, conv2, bn2)], ups
+    [(ct, bn)], head conv, out act), or None when a stage is off the native path: every conv plain (groups 1,
+    dilation 1), every norm an eval BatchNorm with affine parameters, every activation ReLU, the blocks reflect-padded
+    ``ResnetBlock``s without an input conv or dropout."""
+    from .pix2pixhd import GlobalGenerator, ResnetBlock
+    if not isinstance(gen, GlobalGenerator):
+        return None
+    mods = list(gen.model)
+    try:
+        if not (isinstance(mods[0], nn.ReflectionPad2d) and tuple(mods[0].padding) == (3, 3, 3, 3)):
+            return None
+        stem, stem_bn = mods[1], mods[2]
+        if not (type(stem) is nn.Conv2d and stem.kernel_size == (7, 7) and stem.padding == (0, 0)
+                and stem.stride == (1, 1) and stem.groups == 1 and stem.in_channels <= 16
+                and stem.out_channels % 4 == 0 and _affine_bn(stem_bn) and isinstance(mods[3], nn.ReLU)):
+            return None
+        i = 4
+        downs = []
+        while type(mods[i]) is nn.Conv2d:
+            conv, bn, act = mods[i], mods[i + 1], mods[i + 2]
+            if not (_biased_conv(conv, 3, 2, 1, 'zeros') and _affine_bn(bn) and isinstance(act, nn.ReLU)):
+                return None
+            downs.append((conv, bn)); i += 3
+        blocks = []
+        while isinstance(mods[i], ResnetBlock):
+            blk = mods[i]
+            cb = list(blk.conv_block)
+            if blk.in_dim is not None or len(cb) != 7:
+                return None
+            pad1, c1, bn1, act, pad2, c2, bn2 = cb
+            if not (all(isinstance(p, nn.ReflectionPad2d) and tuple(p.padding) == (1, 1, 1, 1) for p in (pad1, pad2))
+                    and all(_biased_conv(c, 3, 1, 0, 'zeros') and c.in_channels == c.out_channels for c in (c1, c2))
+                    and _affine_bn(bn1) and _affine_bn(bn2) and isinstance(act, nn.ReLU)):
+                return None
+            blocks.append((c1, bn1, c2, bn2)); i += 1
+        ups, i = _up_stages(mods, i)
+        if ups is None:
+            return None
+        head, out_act = _head_stage(mods, i)
+        if head is None:
+            return None
+        return stem, stem_bn, downs, blocks, ups, head, out_act
+    except IndexError:
+        return None
+
+
+def generator_in_channels(gen) -> int:
+    """Input channels of a drop-in generator (image + mask: 4 for the shipped models)."""
+    from .pix2pixhd import GlobalGenerator
+    return gen.model[1].in_channels if isinstance(gen, GlobalGenerator) else gen.model[1].ffc.convl2l.in_channels
+
+
 def generator_supported(gen, x) -> bool:
+    glob = _global_layout(gen)
+    if glob is not None:
+        return global_supported(glob, x)
     lay = _generator_layout(gen)
     if lay is None or x.dim() != 4:
         return False
@@ -631,6 +714,18 @@ def generator_supported(gen, x) -> bool:
     if blocks_use_fft(gen) and not plane_ok(h // f, w // f):     # e.g. 1025-wide planes (images above 8192 px)
         return False
     return h // f >= 2 and w // f >= 2      # reflect pad 1 at the bottleneck
+
+
+def global_supported(lay, x) -> bool:
+    """A GlobalGenerator program exists for input ``x``: 4 x H x W with H and W multiples of 2^n_down and at least
+    2 pixels per bottleneck axis (the blocks' reflect padding of 1).  No FFT runs, so no plane-size limit applies."""
+    stem, _bn, downs, _blocks, _ups, _head, _act = lay
+    if x.dim() != 4:
+        return False
+    _b, c, h, w = x.shape
+    f = 2 ** len(downs)
+    return (c == stem.in_channels and h >= 4 and w >= 4 and h % f == 0 and w % f == 0
+            and h // f >= 2 and w // f >= 2)
 
 
 def blocks_use_fft(gen) -> bool:
@@ -1089,36 +1184,14 @@ def build_generator_program(prog: Program, gen, shape, u8_size: Optional[Tuple[i
     ``u8_size=(H0, W0)``: the predict-path variant (SURVEY.md row f1).  Inputs are the decoded bytes "img"
     (B,H0,W0,3) and "mask" (B,H0,W0); ``shape`` is the modulo-padded generator input (B,4,H,W); the output "y0" is
     the inpainted RGB bytes (B,H0,W0,3).  Pre/post-processing lives in the pack and gather kernels."""
+    glob = _global_layout(gen)
+    if glob is not None:
+        return build_global_program(prog, glob, shape, u8_size)
     stem, downs, blocks, ups, out_blk, head, out_act = _generator_layout(gen)
     b, cin, h, w = shape
-    dev = head.weight.device
-    if u8_size is None:
-        prog.inputs["x0"] = tuple(shape)
-    else:
-        h0, w0 = u8_size
-        prog.inputs["img"], prog.inputs["mask"] = (b, h0, w0, 3), (b, h0, w0)
-        prog.dtypes.update(img=torch.uint8, mask=torch.uint8, y0=torch.uint8)
-    conv = stem.ffc.convl2l
-    n0 = conv.out_channels
     s0, b0 = P.bn_scale_shift(stem.bn_l)
-    wst, shst = P.pack_stem(conv.weight, s0, b0, device=dev)
-    X = prog.buf("stem", b, h, w, n0, gemm=True, halo=True)
-    tc_stem = (prog.math == L.MATH_BF16X3 and cin <= 8 and n0 % 8 == 0
-               and os.environ.get("LAMA_B200_STEM", "tc") == "tc")
-    if u8_size is not None and not (tc_stem and cin == 4):
-        raise ValueError("the uint8 predict path needs the tensor-core stem (bf16x3 arithmetic, 4 input channels)")
-    if tc_stem:
-        # tensor-core stem: the 7x7 window of the packed image is 7 contiguous 128-byte K blocks per pixel
-        Pk = prog.buf("stem.packed", b, h + 6, w + 8, 8, gemm=True)
-        if u8_size is None:
-            prog.ops.append(StemPackOp("x0", cin, TV(Pk)))
-        else:
-            prog.ops.append(StemPackU8Op("img", "mask", h0, w0, TV(Pk)))
-        pk = P.pack_stem_windowed(conv.weight, s0, b0, device=dev)
-        prog.ops.append(ConvOp(pk, [TV(Pk, window=8), None], TV(X), tag="stem 7x7 (windowed)+bn+relu"))
-    else:
-        prog.ops.append(StemOp("x0", cin, wst, shst, TV(X)))
-    cl, cg = n0, 0
+    X = emit_stem(prog, stem.ffc.convl2l.weight, s0, b0, shape, u8_size)
+    cl, cg = X.C, 0
     for d in downs:
         X, cl, cg = emit_ffc_bn_act(prog, d, X, cl, cg)
     for blk in blocks:
@@ -1132,10 +1205,80 @@ def build_generator_program(prog: Program, gen, shape, u8_size: Optional[Tuple[i
         # [local | global] channel order of the buffer, so it runs in place like the bottleneck blocks
         ocg = out_blk.conv1.ffc.global_in_num
         X = emit_resnet_block(prog, out_blk, X, X.C - ocg, ocg, in_place=True)
-    if u8_size is not None and not (tc_head and ups and head.out_channels == 3):
+    emit_generator_head(prog, head, out_act, X, tc_head, bool(ups), shape, u8_size)
+
+
+def emit_stem(prog: Program, weight: torch.Tensor, scale: torch.Tensor, shift: torch.Tensor, shape,
+              u8_size: Optional[Tuple[int, int]]) -> Buf:
+    """The generator's inputs and its ReflectionPad2d(3) + 7x7 conv + BN + ReLU stem (ffc.py:314-317,
+    pix2pixhd.py:365-368; a conv bias is folded into ``shift``); returns the stem's output buffer."""
+    b, cin, h, w = shape
+    dev = weight.device
+    if u8_size is None:
+        prog.inputs["x0"] = tuple(shape)
+    else:
+        h0, w0 = u8_size
+        prog.inputs["img"], prog.inputs["mask"] = (b, h0, w0, 3), (b, h0, w0)
+        prog.dtypes.update(img=torch.uint8, mask=torch.uint8, y0=torch.uint8)
+    n0 = weight.shape[0]
+    wst, shst = P.pack_stem(weight, scale, shift, device=dev)
+    X = prog.buf("stem", b, h, w, n0, gemm=True, halo=True)
+    tc_stem = (prog.math == L.MATH_BF16X3 and cin <= 8 and n0 % 8 == 0
+               and os.environ.get("LAMA_B200_STEM", "tc") == "tc")
+    if u8_size is not None and not (tc_stem and cin == 4):
+        raise ValueError("the uint8 predict path needs the tensor-core stem (bf16x3 arithmetic, 4 input channels)")
+    if tc_stem:
+        # tensor-core stem: the 7x7 window of the packed image is 7 contiguous 128-byte K blocks per pixel
+        Pk = prog.buf("stem.packed", b, h + 6, w + 8, 8, gemm=True)
+        if u8_size is None:
+            prog.ops.append(StemPackOp("x0", cin, TV(Pk)))
+        else:
+            prog.ops.append(StemPackU8Op("img", "mask", h0, w0, TV(Pk)))
+        pk = P.pack_stem_windowed(weight, scale, shift, device=dev)
+        prog.ops.append(ConvOp(pk, [TV(Pk, window=8), None], TV(X), tag="stem 7x7 (windowed)+bn+relu"))
+    else:
+        prog.ops.append(StemOp("x0", cin, wst, shst, TV(X)))
+    return X
+
+
+def emit_generator_head(prog: Program, head, out_act: int, X: Buf, tc_head: bool, has_ups: bool, shape,
+                        u8_size: Optional[Tuple[int, int]]):
+    """The head (``emit_head``) and the program output "y0" of a generator program."""
+    b, _cin, h, w = shape
+    if u8_size is not None and not (tc_head and has_ups and head.out_channels == 3):
         raise ValueError("the uint8 predict path needs the tensor-core head with 3 output channels")
-    emit_head(prog, head, out_act, X, tc_head and bool(ups), u8_size)
-    prog.outputs["y0"] = (b, head.out_channels, h, w) if u8_size is None else (b, h0, w0, 3)
+    emit_head(prog, head, out_act, X, tc_head and has_ups, u8_size)
+    prog.outputs["y0"] = (b, head.out_channels, h, w) if u8_size is None else (b, u8_size[0], u8_size[1], 3)
+
+
+def build_global_program(prog: Program, lay, shape, u8_size: Optional[Tuple[int, int]] = None):
+    """LaMa-Regular ``GlobalGenerator`` (pix2pixhd.py:341-436; layout from ``_global_layout``) as one program: the
+    FFC generator's stem, up-sampling tail and head around
+      * 3x3 stride-2 convs with ZERO padding + BN + ReLU (pix2pixhd.py:375-379), conv biases folded into the shifts;
+      * ``ResnetBlock``s in place on one bottleneck buffer X (pix2pixhd.py:47-90):
+            Y = relu(bn1(conv1(reflect_pad(X))))          epilogue writes Y's reflected ring
+            X = X + bn2(conv2(reflect_pad(Y)))            no activation; the residual is the epilogue's addend, and
+                                                          each output pixel reads only its own residual pixel
+    ``u8_size``: the predict-path variant, as in ``build_generator_program``."""
+    stem, stem_bn, downs, blocks, ups, head, out_act = lay
+    b, cin, h, w = shape
+    dev = head.weight.device
+    X = emit_stem(prog, stem.weight, *P.bn_scale_shift(stem_bn, stem.bias), shape, u8_size)
+    for conv, bn in downs:
+        sc, sh = P.bn_scale_shift(bn, conv.bias)
+        Y = prog.buf("down", b, X.H // 2, X.W // 2, conv.out_channels, gemm=True, halo=True)
+        pk = P.pack_conv([(conv.weight, 0, 0, 1)], sc, sh, stride=2, border=L.BORDER_ZERO, act=L.ACT_RELU, device=dev)
+        prog.ops.append(ConvOp(pk, [TV(X), None], TV(Y), tag="down 3x3 s2 (zero border)+bn+relu"))
+        X = Y
+    for c1, bn1, c2, bn2 in blocks:
+        Y = prog.buf("block.y", b, X.H, X.W, X.C, gemm=True, halo=True)
+        pk1 = P.pack_conv([(c1.weight, 0, 0, 1)], *P.bn_scale_shift(bn1, c1.bias), act=L.ACT_RELU, device=dev)
+        prog.ops.append(ConvOp(pk1, [TV(X), None], TV(Y), tag="block conv1+bn1+relu"))
+        pk2 = P.pack_conv([(c2.weight, 0, 0, 1)], *P.bn_scale_shift(bn2, c2.bias), device=dev)
+        prog.ops.append(ConvOp(pk2, [TV(Y), None], TV(X), addend=TV(X), addend_post=True, tag="block conv2+bn2 + x"))
+    tc_head = _tc_head(prog, head, h, w)
+    ups_out = emit_up_tail(prog, ups, X, tc_head)
+    emit_generator_head(prog, head, out_act, ups_out[-1] if ups_out else X, tc_head, bool(ups), shape, u8_size)
 
 
 def _tc_head(prog: Program, head, h: int, w: int) -> bool:

@@ -19,14 +19,20 @@ import torch
 from . import _lib as L
 
 
-def bn_scale_shift(bn: torch.nn.BatchNorm2d) -> Tuple[torch.Tensor, torch.Tensor]:
-    """Eval-mode BN as ``y = scale * x + shift`` (float64).  ffc.py:60,131,243-244,353."""
+def bn_scale_shift(bn: torch.nn.BatchNorm2d, conv_bias: Optional[torch.Tensor] = None
+                   ) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Eval-mode BN as ``y = scale * x + shift`` (float64).  ffc.py:60,131,243-244,353.
+    ``conv_bias``: the bias of the convolution BN follows (pix2pixhd.py convs carry one), folded into the shift:
+    BN(conv(x) + bias) = scale * conv(x) + (shift + scale * bias)."""
     var = bn.running_var.detach().double()
     mean = bn.running_mean.detach().double()
     gamma = bn.weight.detach().double() if bn.weight is not None else torch.ones_like(var)
     beta = bn.bias.detach().double() if bn.bias is not None else torch.zeros_like(var)
     scale = gamma / torch.sqrt(var + bn.eps)
-    return scale, beta - mean * scale
+    shift = beta - mean * scale
+    if conv_bias is not None:
+        shift = shift + scale * conv_bias.detach().double().to(shift.device)
+    return scale, shift
 
 
 @dataclass

@@ -13,6 +13,9 @@ copies of neighbouring batches overlap the kernels (``lama_b200.serving.Generato
 
     python -m lama_b200.predict --model-dir big-lama --indir images/ --outdir out/     # predict.py's file layout
 
+The model directory may hold an FFC generator (big-lama, lama-fourier) or a LaMa-Regular one (lama-regular,
+big-lama-regular: ``pix2pixhd_global``); ``generator_from_config`` builds either.
+
 The arithmetic is the reference's, byte for byte outside the hole and within the generator tolerance (one grey
 level where a truncation boundary is crossed) inside it; ``tests/golden/predict_ngf8_3x45x52.npz`` pins it.
 There is no CPU path: a generator that is not on a CUDA device, or is outside the native path, is an error.
@@ -220,15 +223,40 @@ def generator_kwargs_from_config(cfg: Dict) -> Dict:
     return g
 
 
-def load_generator(model_dir: str, checkpoint: str = "best.ckpt", device: str = "cuda"):
-    """Build the drop-in generator from ``<model_dir>/config.yaml`` and load ``<model_dir>/models/<checkpoint>``
-    (a Lightning checkpoint: generator weights live under the ``generator.`` prefix of ``state_dict`` —
-    saicinpainting/training/trainers/__init__.py:25-30, bin/predict.py:49-59)."""
+def generator_from_config(cfg: Dict):
+    """The drop-in generator a training config describes, as make_generator builds it
+    (saicinpainting/training/modules/__init__.py:7-17): ``ffc_resnet`` -> FFCResNetGenerator (big-lama, lama-fourier),
+    ``pix2pixhd_global`` -> GlobalGenerator (lama-regular, big-lama-regular)."""
+    kind = cfg["generator"]["kind"]
+    if kind == "ffc_resnet":
+        from .modules import FFCResNetGenerator
+        return FFCResNetGenerator(**generator_kwargs_from_config(cfg))
+    if kind == "pix2pixhd_global":
+        from .pix2pixhd import GlobalGenerator
+        return GlobalGenerator(**{k: v for k, v in cfg["generator"].items() if k != "kind"})
+    raise ValueError(f"generator kind {kind!r} has no drop-in generator (ffc_resnet, pix2pixhd_global)")
+
+
+def _read_config(model_dir: str) -> Dict:
     import yaml
-    from .modules import FFCResNetGenerator
     with open(os.path.join(model_dir, "config.yaml")) as f:
-        cfg = yaml.safe_load(f)
-    gen = FFCResNetGenerator(**generator_kwargs_from_config(cfg))
+        return yaml.safe_load(f)
+
+
+def check_refinable(cfg: Dict) -> None:
+    """Refinement optimises the FFC generator's two bottleneck halves (z1, z2; evaluation/refinement.py:128); a
+    ``pix2pixhd_global`` generator has one bottleneck tensor, and the reference cannot refine it either."""
+    kind = cfg["generator"]["kind"]
+    if kind != "ffc_resnet":
+        raise ValueError(f"--refine needs an ffc_resnet generator (big-lama, lama-fourier); this model's generator "
+                         f"kind is {kind!r}")
+
+
+def load_generator(model_dir: str, checkpoint: str = "best.ckpt", device: str = "cuda"):
+    """Build the drop-in generator from ``<model_dir>/config.yaml`` (``generator_from_config``) and load
+    ``<model_dir>/models/<checkpoint>`` (a Lightning checkpoint: generator weights live under the ``generator.``
+    prefix of ``state_dict`` — saicinpainting/training/trainers/__init__.py:25-30, bin/predict.py:49-59)."""
+    gen = generator_from_config(_read_config(model_dir))
     state = torch.load(os.path.join(model_dir, "models", checkpoint), map_location="cpu", weights_only=False)
     sd = state.get("state_dict", state)
     sd = {k[len("generator."):]: v for k, v in sd.items() if k.startswith("generator.")} or sd
@@ -315,6 +343,8 @@ def main(argv=None):
     # takes its share of the files; single-process runs see rank 0 of 1
     rank, world = int(os.environ.get("RANK", "0")), int(os.environ.get("WORLD_SIZE", "1"))
     device = f"cuda:{os.environ.get('LOCAL_RANK', '0')}"
+    if a.refine:
+        check_refinable(_read_config(a.model_dir))
     gen = load_generator(a.model_dir, a.checkpoint, device=device)
     if a.refine:
         from .refine import BatchedRefiner

@@ -29,7 +29,7 @@ class GeneratorPipeline:
         dev = device if device is not None else next(generator.parameters()).device
         assert dev.type == "cuda", "GeneratorPipeline needs the generator on a CUDA device"
         self.device, self.depth = dev, depth
-        cin = generator.model[1].ffc.convl2l.in_channels
+        cin = E.generator_in_channels(generator)
         hp, wp = (-(-height // pad_mod) * pad_mod, -(-width // pad_mod) * pad_mod) if u8 else (height, width)
         probe = torch.empty(batch, cin, hp, wp, device=dev)
         if not E.generator_supported(generator, probe):

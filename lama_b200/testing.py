@@ -22,6 +22,17 @@ BIG_LAMA_KWARGS = dict(
 )
 
 
+# configs/training/generator/pix2pixhd_global_sigmoid.yaml (lama-regular.yaml:29) and big-lama-regular.yaml:3-11:
+# GlobalGenerator (lama_b200.pix2pixhd) kwargs.
+LAMA_REGULAR_KWARGS = dict(input_nc=4, output_nc=3, ngf=64, n_downsampling=3, n_blocks=9, conv_kind="default",
+                           add_out_act="sigmoid")
+BIG_LAMA_REGULAR_KWARGS = dict(LAMA_REGULAR_KWARGS, n_blocks=15)
+
+
+def small_regular_kwargs(ngf=8, n_blocks=2, n_downsampling=3):
+    return dict(LAMA_REGULAR_KWARGS, ngf=ngf, n_blocks=n_blocks, n_downsampling=n_downsampling)
+
+
 def small_lama_kwargs(ngf=8, n_blocks=2, n_downsampling=3):
     kw = {k: (dict(v) if isinstance(v, dict) else v) for k, v in BIG_LAMA_KWARGS.items()}
     kw.update(ngf=ngf, n_blocks=n_blocks, n_downsampling=n_downsampling)
