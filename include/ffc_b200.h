@@ -38,8 +38,9 @@
 extern "C" {
 #endif
 
-#define FFCB_VERSION 114 /* 0.1.4: ffcb_relu_mask_pack, ffcb_relu_bwd_bits (0.1.3: ffcb_refine_l1_grad; 0.1.2: ffcb_add,
-                            ffcb_head_bwd7; 0.1.1: ffcb_tensor gained cg / tile / sg) */
+#define FFCB_VERSION 115 /* 0.1.5: ffcb_head_bwd7_bits, ffcb_relu_mask_pack_rows, ffcb_relu_bwd_bits_rows,
+                            ffcb_head_gather7_rows (0.1.4: ffcb_relu_mask_pack, ffcb_relu_bwd_bits; 0.1.3:
+                            ffcb_refine_l1_grad; 0.1.2: ffcb_add, ffcb_head_bwd7; 0.1.1: ffcb_tensor gained cg / tile / sg) */
 
 enum {
   FFCB_OK = 0,
@@ -272,6 +273,16 @@ int ffcb_relu_mask_pack(const ffcb_tensor* y, uint32_t* bits, ffcb_stream_t stre
 int ffcb_relu_bwd_bits(const ffcb_tensor* dy, const uint32_t* bits, const ffcb_tensor* out, ffcb_stream_t stream);
 
 /*
+ * Row bands of a bit mask (the banded up-sampling tail of the refinement step, lama_b200/banded.py): `bits` is the mask
+ * of a whole plane of H rows, B*H*W*nw words laid out as above, and the view (`y`, resp. `dy` / `out`) holds its rows
+ * [row0, row0 + view.H) (view.W = the plane's W).  With H = view.H and row0 = 0 these are ffcb_relu_mask_pack and
+ * ffcb_relu_bwd_bits.  For B > 1 a band's words are not contiguous: image b's rows start at word b*H*W*nw.
+ */
+int ffcb_relu_mask_pack_rows(const ffcb_tensor* y, uint32_t* bits, int H, int row0, ffcb_stream_t stream);
+int ffcb_relu_bwd_bits_rows(const ffcb_tensor* dy, const uint32_t* bits, int H, int row0, const ffcb_tensor* out,
+                            ffcb_stream_t stream);
+
+/*
  * Input gradients through the generator's rear (residual blocks -> ConcatTupleLayer -> up-sampling tail -> head,
  * ffc.py:345-363; what evaluation/refinement.py:137-167 back-propagates through on every Adam step) as one program:
  *   ffcb_add:       out = a + b elementwise over the whole padded extent (interior and ring) of three views of one
@@ -290,6 +301,18 @@ int ffcb_relu_bwd_bits(const ffcb_tensor* dy, const uint32_t* bits, const ffcb_t
 int ffcb_add(const ffcb_tensor* a, const ffcb_tensor* b, const ffcb_tensor* out, ffcb_stream_t stream);
 int ffcb_head_bwd7(const float* y_nchw, const float* dy_nchw, int B, int N, int H, int W, const float* w, int act,
                    const ffcb_tensor* mask, const ffcb_tensor* out, ffcb_stream_t stream);
+/*
+ * ffcb_head_bwd7_bits: ffcb_head_bwd7 with the mask read as bits (ffcb_relu_mask_pack of the last up-sampling output,
+ * B*H*W*ceil(Cin/32) words of the whole plane), writing rows [row0, row0 + out.H) of the result into out (B, rows, W,
+ * Cin).  y, dy are the whole NCHW planes: a band reads the gradient rows its 7x7 windows reach and folds the
+ * reflection only at the plane's own top and bottom rows, so every pixel gets the operands, and the summation order,
+ * of ffcb_head_bwd7 — the two are equal bit for bit.
+ * ffcb_head_gather7_rows: ffcb_head_gather7 writing rows [row0, row0 + q.H) of an NCHW output of H rows.
+ */
+int ffcb_head_bwd7_bits(const float* y_nchw, const float* dy_nchw, int B, int N, int H, int W, const float* w, int act,
+                        const uint32_t* mask_bits, int row0, const ffcb_tensor* out, ffcb_stream_t stream);
+int ffcb_head_gather7_rows(const ffcb_tensor* q, const float* bias, int N, int act, float* y_nchw, int H, int row0,
+                           ffcb_stream_t stream);
 
 /*
  * Gradient of the refinement loss w.r.t. the prediction (evaluation/refinement.py:75-84 _l1_loss, 19-26 _pyrdown,

@@ -17,7 +17,7 @@ ACT_NONE, ACT_RELU, ACT_SIGMOID, ACT_TANH = 0, 1, 2, 3
 BORDER_ZERO, BORDER_REFLECT = 0, 1
 MATH_FP32, MATH_BF16X3 = 0, 1
 MAX_KSEG = 64
-VERSION = 114
+VERSION = 115
 
 
 class Tensor(C.Structure):
@@ -70,6 +70,12 @@ SIGNATURES = {
     "ffcb_add": (C.c_int, [_PT, _PT, _PT, C.c_void_p]),
     "ffcb_head_bwd7": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                  _PT, _PT, C.c_void_p]),
+    "ffcb_head_bwd7_bits": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                      C.c_int, C.c_void_p, C.c_int, _PT, C.c_void_p]),
+    "ffcb_relu_mask_pack_rows": (C.c_int, [_PT, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
+    "ffcb_relu_bwd_bits_rows": (C.c_int, [_PT, C.c_void_p, C.c_int, C.c_int, _PT, C.c_void_p]),
+    "ffcb_head_gather7_rows": (C.c_int, [_PT, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int,
+                                         C.c_void_p]),
     "ffcb_refine_l1_grad": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p] + [C.c_int] * 6 + [C.c_void_p] * 7
                             + [C.c_void_p]),
     "ffcb_launch_count": (C.c_longlong, []),

@@ -76,17 +76,22 @@ int nhwc_to_nchw(const ffcb_tensor*, float*, cudaStream_t);
 int fill_reflect_border(const ffcb_tensor*, cudaStream_t);
 int stem_pack(const float*, int, int, int, int, const ffcb_tensor*, cudaStream_t);
 int head_gather7(const ffcb_tensor*, const float*, int, int, float*, cudaStream_t);
+int head_gather7_rows(const ffcb_tensor*, const float*, int, int, float*, int, int, cudaStream_t);
 int stem_pack_u8(const uint8_t*, const uint8_t*, int, int, int, const ffcb_tensor*, cudaStream_t);
 int head_gather7_blend_u8(const ffcb_tensor*, const float*, int, const uint8_t*, const uint8_t*, int, int, uint8_t*,
                           cudaStream_t);
 int relu_bwd(const ffcb_tensor*, const ffcb_tensor*, const ffcb_tensor*, cudaStream_t);
 int relu_mask_pack(const ffcb_tensor*, uint32_t*, cudaStream_t);
 int relu_bwd_bits(const ffcb_tensor*, const uint32_t*, const ffcb_tensor*, cudaStream_t);
+int relu_mask_pack_rows(const ffcb_tensor*, uint32_t*, int, int, cudaStream_t);
+int relu_bwd_bits_rows(const ffcb_tensor*, const uint32_t*, int, int, const ffcb_tensor*, cudaStream_t);
 int fold_reflect_border(const ffcb_tensor*, const ffcb_tensor*, int, const ffcb_tensor*, int, const ffcb_tensor*,
                         cudaStream_t);
 int add(const ffcb_tensor*, const ffcb_tensor*, const ffcb_tensor*, cudaStream_t);
 int head_bwd7(const float*, const float*, int, int, int, int, const float*, int, const ffcb_tensor*, const ffcb_tensor*,
               cudaStream_t);
+int head_bwd7_bits(const float*, const float*, int, int, int, int, const float*, int, const uint32_t*, int,
+                   const ffcb_tensor*, cudaStream_t);
 int refine_l1_grad(const float*, const float*, const float*, int, int, int, int, int, int, const float*, const float*,
                    const float*, const float*, float*, float*, float*, cudaStream_t);
 
@@ -234,6 +239,25 @@ int ffcb_add(const ffcb_tensor* a, const ffcb_tensor* b, const ffcb_tensor* out,
 int ffcb_head_bwd7(const float* y_nchw, const float* dy_nchw, int B, int N, int H, int W, const float* w, int act,
                    const ffcb_tensor* mask, const ffcb_tensor* out, ffcb_stream_t stream) {
   return head_bwd7(y_nchw, dy_nchw, B, N, H, W, w, act, mask, out, (cudaStream_t)stream);
+}
+
+int ffcb_head_bwd7_bits(const float* y_nchw, const float* dy_nchw, int B, int N, int H, int W, const float* w,
+                        int act, const uint32_t* mask_bits, int row0, const ffcb_tensor* out, ffcb_stream_t stream) {
+  return head_bwd7_bits(y_nchw, dy_nchw, B, N, H, W, w, act, mask_bits, row0, out, (cudaStream_t)stream);
+}
+
+int ffcb_relu_mask_pack_rows(const ffcb_tensor* y, uint32_t* bits, int H, int row0, ffcb_stream_t stream) {
+  return relu_mask_pack_rows(y, bits, H, row0, (cudaStream_t)stream);
+}
+
+int ffcb_relu_bwd_bits_rows(const ffcb_tensor* dy, const uint32_t* bits, int H, int row0, const ffcb_tensor* out,
+                            ffcb_stream_t stream) {
+  return relu_bwd_bits_rows(dy, bits, H, row0, out, (cudaStream_t)stream);
+}
+
+int ffcb_head_gather7_rows(const ffcb_tensor* q, const float* bias, int N, int act, float* y_nchw, int H, int row0,
+                           ffcb_stream_t stream) {
+  return head_gather7_rows(q, bias, N, act, y_nchw, H, row0, (cudaStream_t)stream);
 }
 
 int ffcb_refine_l1_grad(const float* pred, const float* image, const float* mask, int B, int C, int Hp, int Wp, int H0,

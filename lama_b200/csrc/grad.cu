@@ -16,7 +16,8 @@
 // build_rear_grad_program):
 //   ffcb_add                  out = a + b over the padded extent (the block identity X + Y2, ffc.py:288, with Y2 kept)
 //   ffcb_head_bwd7            adjoint of ReflectionPad2d(3) + Conv2d 7x7 + act (ffc.py:360-363), fused with the ReLU
-//                             mask of the last up-sampling stage (ffc.py:350-354)
+//                             mask of the last up-sampling stage (ffc.py:350-354); ffcb_head_bwd7_bits reads that mask
+//                             as bits and may write a row band of the plane (the banded up-sampling tail)
 #include <stdint.h>
 
 #include "common.cuh"
@@ -56,7 +57,14 @@ __global__ void relu_bwd_kernel(View dy, View y, View out) {
 
 // channels-last views: one warp per (pixel, 32-channel word), lane l tests channel 32w + l and __ballot_sync builds
 // the word (a warp reads 32 adjacent channels: 128 contiguous bytes per fp32 plane, 64 per bf16 plane)
-__global__ void relu_mask_pack_cl_kernel(View y, uint32_t* __restrict__ bits, int nw) {
+// Row bands: the words of a view of rows [row0, row0 + y.H) of a plane of hb rows live at
+// ((b*hb + row0 + y)*W + x)*nw + c/32 — a band of a whole-plane mask buffer; hb = y.H, row0 = 0 is the whole plane.
+__device__ __forceinline__ long long band_word(long long p, int W, int H, int hb, int row0, int nw) {
+  const long long row = p / W, b = row / H;
+  return ((b * hb + row0 + (row - b * H)) * W + p % W) * nw;
+}
+
+__global__ void relu_mask_pack_cl_kernel(View y, uint32_t* __restrict__ bits, int nw, int hb, int row0) {
   const long long total = (long long)y.B * y.H * y.W * nw;
   const int lane = threadIdx.x & 31;
   const long long nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
@@ -68,13 +76,13 @@ __global__ void relu_mask_pack_cl_kernel(View y, uint32_t* __restrict__ bits, in
     const int c = 32 * w + lane;
     const bool on = c < y.C && load1(y, pix_off(y, b, yy, x) + c) > 0.f;
     const unsigned word = __ballot_sync(0xffffffffu, on);
-    if (lane == 0) bits[i] = word;
+    if (lane == 0) bits[band_word(p, y.W, y.H, hb, row0, nw) + w] = word;
   }
 }
 
 // channel-group planar / tile-blocked views: one thread per (pixel, word), pixels fastest so that neighbouring threads
 // read neighbouring pixels of one group plane; 4-channel loads never straddle a group (C % 4 == 0, cg in {4, 8})
-__global__ void relu_mask_pack_cg_kernel(View y, uint32_t* __restrict__ bits, int nw) {
+__global__ void relu_mask_pack_cg_kernel(View y, uint32_t* __restrict__ bits, int nw, int hb, int row0) {
   const long long npix = (long long)y.B * y.H * y.W;
   const long long total = npix * nw;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
@@ -88,12 +96,12 @@ __global__ void relu_mask_pack_cg_kernel(View y, uint32_t* __restrict__ bits, in
       word |= ((unsigned)(a.x > 0.f) | (unsigned)(a.y > 0.f) << 1 | (unsigned)(a.z > 0.f) << 2 |
                (unsigned)(a.w > 0.f) << 3) << k;
     }
-    bits[p * nw + w] = word;
+    bits[band_word(p, y.W, y.H, hb, row0, nw) + w] = word;
   }
 }
 
 // relu_bwd_kernel with the mask read from the packed words: the same loop order, loads and stores
-__global__ void relu_bwd_bits_kernel(View dy, const uint32_t* __restrict__ bits, int nw, View out) {
+__global__ void relu_bwd_bits_kernel(View dy, const uint32_t* __restrict__ bits, int nw, int hb, int row0, View out) {
   const int c4 = out.C / 4;
   const long long total = (long long)out.B * out.H * out.W * c4;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
@@ -104,7 +112,7 @@ __global__ void relu_bwd_bits_kernel(View dy, const uint32_t* __restrict__ bits,
     const int yy = (int)((p / out.W) % out.H);
     const int b = (int)(p / ((long long)out.W * out.H));
     const float4 g = load4g(dy, b, yy, x, 4 * q);
-    const unsigned m = __ldg(bits + p * nw + (q >> 3)) >> (4 * (q & 7));     // channels 4q .. 4q+3
+    const unsigned m = __ldg(bits + band_word(p, out.W, out.H, hb, row0, nw) + (q >> 3)) >> (4 * (q & 7));  // 4q..4q+3
     store4g(out, b, yy, x, 4 * q,
             make_float4((m & 1u) ? g.x : 0.f, (m & 2u) ? g.y : 0.f, (m & 4u) ? g.z : 0.f, (m & 8u) ? g.w : 0.f));
   }
@@ -185,12 +193,13 @@ __device__ __forceinline__ void fma4(float4& a, float g, const float4& w) {
 __global__ void __launch_bounds__(HB_THREADS) head_bwd7_kernel(const float* __restrict__ y, const float* __restrict__ dy,
                                                                int N, int H, int W, int Cin,
                                                                const float* __restrict__ w, int act, View mask,
+                                                               const uint32_t* __restrict__ mbits, int row0, int hout,
                                                                View out, int nchunk) {
   __shared__ float g_s[4][HB_GR][HB_GC];
   __shared__ __align__(16) float w_s[4 * 49 * HB_CC];
   const int b = blockIdx.z / nchunk, c0 = (blockIdx.z % nchunk) * HB_CC;
   const int cc = min(HB_CC, Cin - c0);
-  const int y0 = blockIdx.y * HB_TH, x0 = blockIdx.x * HB_TW;
+  const int y0 = row0 + blockIdx.y * HB_TH, x0 = blockIdx.x * HB_TW;     // plane rows; out holds [row0, row0+hout)
   const int tid = threadIdx.x;
   for (int i = tid; i < N * 49 * HB_CC; i += HB_THREADS) {           // w: [N][49][Cin] -> [N][49][HB_CC]
     const int c = i % HB_CC, nt = i / HB_CC;
@@ -229,7 +238,7 @@ __global__ void __launch_bounds__(HB_THREADS) head_bwd7_kernel(const float* __re
   }
   if (4 * q >= cc) return;
   const int yy = y0 + ty;
-  if (yy >= H) return;
+  if (yy >= row0 + hout) return;
   int rows[3], nr = 1;
   rows[0] = yy + 3;
   if (yy >= 1 && yy <= 3) rows[nr++] = 3 - yy;
@@ -257,9 +266,16 @@ __global__ void __launch_bounds__(HB_THREADS) head_bwd7_kernel(const float* __re
             }
           }
       }
-    const float4 m = load4g(mask, b, yy, xx, c0 + 4 * q);
-    store4g(out, b, yy, xx, c0 + 4 * q,
-            make_float4(m.x > 0.f ? r.x : 0.f, m.y > 0.f ? r.y : 0.f, m.z > 0.f ? r.z : 0.f, m.w > 0.f ? r.w : 0.f));
+    bool on[4];
+    if (mbits != nullptr) {          // words of the whole plane; channels c0+4q .. +3 share one word (c0 % 32 == 0)
+      const unsigned m = __ldg(mbits + (((long long)b * H + yy) * W + xx) * ((Cin + 31) / 32) + (c0 >> 5)) >> (4 * q);
+      on[0] = m & 1u; on[1] = m & 2u; on[2] = m & 4u; on[3] = m & 8u;
+    } else {
+      const float4 m = load4g(mask, b, yy - row0, xx, c0 + 4 * q);
+      on[0] = m.x > 0.f; on[1] = m.y > 0.f; on[2] = m.z > 0.f; on[3] = m.w > 0.f;
+    }
+    store4g(out, b, yy - row0, xx, c0 + 4 * q,
+            make_float4(on[0] ? r.x : 0.f, on[1] ? r.y : 0.f, on[2] ? r.z : 0.f, on[3] ? r.w : 0.f));
   }
 }
 
@@ -280,37 +296,50 @@ int relu_bwd(const ffcb_tensor* dy, const ffcb_tensor* y, const ffcb_tensor* out
   return FFCB_OK;
 }
 
-int relu_mask_pack(const ffcb_tensor* y, uint32_t* bits, cudaStream_t stream) {
+int relu_mask_pack_rows(const ffcb_tensor* y, uint32_t* bits, int hb, int row0, cudaStream_t stream) {
   int rc;
   if ((rc = check_tensor(y, "relu_mask_pack.y", true))) return rc;
+  FFCB_REQUIRE(row0 >= 0 && row0 + y->H <= hb, "relu_mask_pack: rows [%d, %d) outside a plane of %d rows", row0,
+               row0 + y->H, hb);
   const long long npix = (long long)y->B * y->H * y->W;
   if (npix * y->C == 0) return FFCB_OK;
   FFCB_REQUIRE(bits != nullptr && ((uintptr_t)bits % 4) == 0, "relu_mask_pack: bits must be a 4-byte aligned pointer");
   const int nw = (y->C + 31) / 32;
   const View v = make_view(*y);
   if (v.cg) {
-    relu_mask_pack_cg_kernel<<<grid_for(npix * nw), 256, 0, stream>>>(v, bits, nw);
+    relu_mask_pack_cg_kernel<<<grid_for(npix * nw), 256, 0, stream>>>(v, bits, nw, hb, row0);
     FFCB_LAUNCH_CHECK("relu_mask_pack_cg_kernel");
   } else {
-    relu_mask_pack_cl_kernel<<<grid_for(npix * nw * 32), 256, 0, stream>>>(v, bits, nw);
+    relu_mask_pack_cl_kernel<<<grid_for(npix * nw * 32), 256, 0, stream>>>(v, bits, nw, hb, row0);
     FFCB_LAUNCH_CHECK("relu_mask_pack_cl_kernel");
   }
   return FFCB_OK;
 }
 
-int relu_bwd_bits(const ffcb_tensor* dy, const uint32_t* bits, const ffcb_tensor* out, cudaStream_t stream) {
+int relu_mask_pack(const ffcb_tensor* y, uint32_t* bits, cudaStream_t stream) {
+  return relu_mask_pack_rows(y, bits, y == nullptr ? 0 : y->H, 0, stream);
+}
+
+int relu_bwd_bits_rows(const ffcb_tensor* dy, const uint32_t* bits, int hb, int row0, const ffcb_tensor* out,
+                       cudaStream_t stream) {
   int rc;
   if ((rc = check_tensor(dy, "relu_bwd_bits.dy", true)) || (rc = check_tensor(out, "relu_bwd_bits.out", true)))
     return rc;
+  FFCB_REQUIRE(row0 >= 0 && row0 + out->H <= hb, "relu_bwd_bits: rows [%d, %d) outside a plane of %d rows", row0,
+               row0 + out->H, hb);
   FFCB_REQUIRE(dy->B == out->B && dy->H == out->H && dy->W == out->W && dy->C == out->C,
                "relu_bwd_bits: shapes differ");
   const long long total = (long long)out->B * out->H * out->W * (out->C / 4);
   if (total == 0) return FFCB_OK;
   FFCB_REQUIRE(bits != nullptr && ((uintptr_t)bits % 4) == 0, "relu_bwd_bits: bits must be a 4-byte aligned pointer");
-  relu_bwd_bits_kernel<<<grid_for(total), 256, 0, stream>>>(make_view(*dy), bits, (out->C + 31) / 32,
+  relu_bwd_bits_kernel<<<grid_for(total), 256, 0, stream>>>(make_view(*dy), bits, (out->C + 31) / 32, hb, row0,
                                                             make_view(*out));
   FFCB_LAUNCH_CHECK("relu_bwd_bits_kernel");
   return FFCB_OK;
+}
+
+int relu_bwd_bits(const ffcb_tensor* dy, const uint32_t* bits, const ffcb_tensor* out, cudaStream_t stream) {
+  return relu_bwd_bits_rows(dy, bits, out == nullptr ? 0 : out->H, 0, out, stream);
 }
 
 int fold_reflect_border(const ffcb_tensor* gpad, const ffcb_tensor* add0, int add0_c0, const ffcb_tensor* add1,
@@ -372,8 +401,32 @@ int head_bwd7(const float* y, const float* dy, int B, int N, int H, int W, const
   const int nchunk = (out->C + HB_CC - 1) / HB_CC;
   FFCB_REQUIRE((long long)B * nchunk <= 65535, "head_bwd7: batch %d too large", B);
   dim3 grid((W + HB_TW - 1) / HB_TW, (H + HB_TH - 1) / HB_TH, B * nchunk);
-  head_bwd7_kernel<<<grid, HB_THREADS, 0, stream>>>(y, dy, N, H, W, out->C, w, act, make_view(*mask),
+  head_bwd7_kernel<<<grid, HB_THREADS, 0, stream>>>(y, dy, N, H, W, out->C, w, act, make_view(*mask), nullptr, 0, H,
                                                      make_view(*out), nchunk);
+  FFCB_LAUNCH_CHECK("head_bwd7_kernel");
+  return FFCB_OK;
+}
+
+int head_bwd7_bits(const float* y, const float* dy, int B, int N, int H, int W, const float* w, int act,
+                   const uint32_t* mask_bits, int row0, const ffcb_tensor* out, cudaStream_t stream) {
+  int rc;
+  if ((rc = check_tensor(out, "head_bwd7_bits.out"))) return rc;
+  FFCB_REQUIRE(N >= 1 && N <= 4, "head_bwd7_bits: N=%d outside [1,4]", N);
+  FFCB_REQUIRE(act == FFCB_ACT_NONE || act == FFCB_ACT_SIGMOID || act == FFCB_ACT_TANH,
+               "head_bwd7_bits: activation %d is not none / sigmoid / tanh", act);
+  FFCB_REQUIRE(H >= 4 && W >= 4, "head_bwd7_bits: ReflectionPad2d(3) needs H, W >= 4 (got %dx%d)", H, W);
+  FFCB_REQUIRE(out->B == B && out->W == W && row0 >= 0 && row0 + out->H <= H && !out->window,
+               "head_bwd7_bits: out must be a (B, rows, W, Cin) view of rows [row0, row0+rows) of the %dx%d plane",
+               H, W);
+  FFCB_REQUIRE(y != nullptr && dy != nullptr && w != nullptr && mask_bits != nullptr &&
+                   ((uintptr_t)mask_bits % 4) == 0,
+               "head_bwd7_bits: null or misaligned pointer");
+  if ((long long)B * out->H * W * out->C == 0) return FFCB_OK;
+  const int nchunk = (out->C + HB_CC - 1) / HB_CC;
+  FFCB_REQUIRE((long long)B * nchunk <= 65535, "head_bwd7_bits: batch %d too large", B);
+  dim3 grid((W + HB_TW - 1) / HB_TW, (out->H + HB_TH - 1) / HB_TH, B * nchunk);
+  head_bwd7_kernel<<<grid, HB_THREADS, 0, stream>>>(y, dy, N, H, W, out->C, w, act, null_view(), mask_bits, row0,
+                                                     out->H, make_view(*out), nchunk);
   FFCB_LAUNCH_CHECK("head_bwd7_kernel");
   return FFCB_OK;
 }

@@ -326,8 +326,9 @@ __global__ void reflect_ring_kernel(View t) {
 // Head gather: y[b,n,y,x] = act(bias[n] + sum_kx q[b,y,reflect(x+kx-3),n*7+kx]).  One CTA = 128 consecutive
 // pixels of a row; the (128+6) x 7N partial sums are staged through shared memory (row pitch 7N+1: conflict-free).
 constexpr int GT = 128;
+// Output rows [row0, row0 + q.H) of an NCHW plane of hout rows (hout = q.H, row0 = 0: the whole plane).
 __global__ void __launch_bounds__(GT) head_gather7_kernel(View q, const float* __restrict__ bias, int N, int act,
-                                                          float* __restrict__ y_out) {
+                                                          float* __restrict__ y_out, int hout, int row0) {
   extern __shared__ float tile[];
   const int nq = 7 * N, pitch = nq + 1;
   const int tiles_x = (q.W + GT - 1) / GT;
@@ -344,7 +345,7 @@ __global__ void __launch_bounds__(GT) head_gather7_kernel(View q, const float* _
     float acc = bias ? __ldg(bias + n) : 0.f;
 #pragma unroll
     for (int kx = 0; kx < 7; ++kx) acc += tile[(threadIdx.x + kx) * pitch + n * 7 + kx];
-    y_out[(((long long)b * N + n) * q.H + y) * q.W + x] = apply_act(acc, act);
+    y_out[(((long long)b * N + n) * hout + row0 + y) * q.W + x] = apply_act(acc, act);
   }
 }
 
@@ -460,18 +461,25 @@ int head_gather7_blend_u8(const ffcb_tensor* q, const float* bias, int act, cons
   return FFCB_OK;
 }
 
-int head_gather7(const ffcb_tensor* q, const float* bias, int N, int act, float* y, cudaStream_t stream) {
+int head_gather7_rows(const ffcb_tensor* q, const float* bias, int N, int act, float* y, int hout, int row0,
+                      cudaStream_t stream) {
   int rc;
   if ((rc = check_tensor(q, "head_gather7.q"))) return rc;
+  FFCB_REQUIRE(row0 >= 0 && row0 + q->H <= hout, "head_gather7: rows [%d, %d) outside an output of %d rows", row0,
+               row0 + q->H, hout);
   FFCB_REQUIRE(y != nullptr, "head_gather7: null output");
   FFCB_REQUIRE(N >= 1 && N <= 4 && q->C >= 7 * N, "head_gather7: need 1 <= N <= 4 and q.C >= 7N (N=%d, C=%d)", N, q->C);
   FFCB_REQUIRE(q->W >= 4 && q->B <= 65535, "head_gather7: W >= 4 and B <= 65535 required");
   if (q->B == 0) return FFCB_OK;
   dim3 grid(((q->W + GT - 1) / GT) * q->H, q->B);
   const size_t smem = sizeof(float) * (GT + 6) * (7 * N + 1);
-  head_gather7_kernel<<<grid, GT, smem, stream>>>(make_view(*q), bias, N, act, y);
+  head_gather7_kernel<<<grid, GT, smem, stream>>>(make_view(*q), bias, N, act, y, hout, row0);
   FFCB_LAUNCH_CHECK("head_gather7_kernel");
   return FFCB_OK;
+}
+
+int head_gather7(const ffcb_tensor* q, const float* bias, int N, int act, float* y, cudaStream_t stream) {
+  return head_gather7_rows(q, bias, N, act, y, q == nullptr ? 0 : q->H, 0, stream);
 }
 
 int head_conv7(const ffcb_tensor* in, const float* w, const float* bias, int N, int act, float* y,

@@ -1162,6 +1162,10 @@ def build_module_program(module, kind: str, shapes: Sequence[Optional[Tuple[int,
     elif kind.startswith("generator_refine_bits:"):     # the same step, ReLU masks kept as bits (relu_masks="bits")
         h0, w0 = (int(v) for v in kind.split(":")[1].split("x"))
         build_refine_program(prog, module, shapes[0], shapes[1], (h0, w0), relu_masks="bits")
+    elif kind.startswith("generator_refine_bits_banded:"):   # bits, and the up-sampling tail in row bands
+        from .banded import build_refine_banded_program
+        h0, w0 = (int(v) for v in kind.split(":")[1].split("x"))
+        build_refine_banded_program(prog, module, shapes[0], shapes[1], (h0, w0))
     elif kind.startswith("generator_u8"):            # "generator_u8:<pad modulo>", shapes = (img, mask)
         mod = int(kind.split(":")[1]) if ":" in kind else 8
         b, h0, w0, _ = shapes[0]
@@ -1364,7 +1368,19 @@ def emit_rear_forward(prog: Program, gen, sl: Tuple[int, ...], sg: Tuple[int, ..
     """Forward part of the rear programs: inputs x0, x1 (z1, z2) -> output y0 (pred).  Per block conv1 -> Y1, conv2 ->
     its own Y2 (kept: its ReLU mask is read by the backward, which the fused residual epilogue's X + Y2 would not give
     back), X <- X + Y2 (ffcb_add); then the generator program's tail.  Returns what the backward reads."""
-    _stem, _downs, blocks, ups, _out_blk, head, out_act = _generator_layout(gen)
+    _stem, _downs, _blocks, ups, _out_blk, head, out_act = _generator_layout(gen)
+    X, saved = emit_rear_blocks(prog, gen, sl, sg)
+    H, W = X.H * 2 ** len(ups), X.W * 2 ** len(ups)
+    ups_out = emit_up_tail(prog, ups, X, _tc_head(prog, head, H, W))
+    emit_head(prog, head, out_act, ups_out[-1], _tc_head(prog, head, H, W))
+    prog.outputs["y0"] = (sl[0], head.out_channels, H, W)
+    return dict(sl=tuple(sl), sg=tuple(sg), saved=saved, ups_out=ups_out)
+
+
+def emit_rear_blocks(prog: Program, gen, sl: Tuple[int, ...], sg: Tuple[int, ...]) -> Tuple[Buf, list]:
+    """The inputs x0, x1 (z1, z2) and the residual blocks of the rear's forward; returns the bottleneck buffer and, per
+    block, (block, Y1, Y2) for the backward."""
+    blocks = _generator_layout(gen)[2]
     b, cl, h, w = sl
     cg = sg[1]
     prog.inputs.update(x0=tuple(sl), x1=tuple(sg))
@@ -1377,11 +1393,7 @@ def emit_rear_forward(prog: Program, gen, sl: Tuple[int, ...], sg: Tuple[int, ..
         Y2, _, _ = emit_ffc_bn_act(prog, blk.conv2, Y1, cl, cg)
         prog.ops.append(AddOp(TV(X), TV(Y2), TV(X)))
         saved.append((blk, Y1, Y2))
-    H, W = X.H * 2 ** len(ups), X.W * 2 ** len(ups)
-    ups_out = emit_up_tail(prog, ups, X, _tc_head(prog, head, H, W))
-    emit_head(prog, head, out_act, ups_out[-1], _tc_head(prog, head, H, W))
-    prog.outputs["y0"] = (b, head.out_channels, H, W)
-    return dict(sl=tuple(sl), sg=tuple(sg), saved=saved, ups_out=ups_out)
+    return X, saved
 
 
 def emit_rear_backward(prog: Program, gen, fwd: dict, dy: str):
@@ -1392,7 +1404,7 @@ def emit_rear_backward(prog: Program, gen, fwd: dict, dy: str):
     below -> the blocks in reverse, each as two FFC_BN_ACT backwards with the identity path added by the second."""
     _stem, _downs, _blocks, ups, _out_blk, head, out_act = _generator_layout(gen)
     sl, sg, saved, ups_out = fwd["sl"], fwd["sg"], fwd["saved"], fwd["ups_out"]
-    b, cl, cg = sl[0], sl[1], sg[1]
+    b = sl[0]
     H, W = ups_out[-1].H, ups_out[-1].W
     dev = head.weight.device
     n = head.out_channels
@@ -1401,9 +1413,7 @@ def emit_rear_backward(prog: Program, gen, fwd: dict, dy: str):
     prog.ops.append(HeadBwdOp("y0", dy, wh, n, out_act, TV(ups_out[-1]), TV(D)))
     for k in reversed(range(len(ups))):
         ct, bn = ups[k]
-        sc, _ = P.bn_scale_shift(bn)
-        wadj = ct.weight.detach().double() * sc.double()[None, :, None, None]       # [Cin_ct, Cout_ct, 3, 3]
-        pk = P.pack_conv([(wadj, 0, 0, 1)], None, None, stride=2, border=L.BORDER_ZERO, device=dev)
+        pk = pack_up_adjoint(ct, bn, dev)
         hi, wi = ups_out[k].H // 2, ups_out[k].W // 2
         if k > 0:
             E_ = prog.buf("grad.up_in", b, hi, wi, ct.in_channels)
@@ -1413,6 +1423,20 @@ def emit_rear_backward(prog: Program, gen, fwd: dict, dy: str):
         else:
             DX = prog.buf("grad.dx", b, hi, wi, ct.in_channels)
             prog.ops.append(ConvOp(pk, [TV(D), None], TV(DX), tag=f"grad: convT{k}^T (stride 2)"))
+    emit_rear_blocks_backward(prog, saved, DX, sl, sg)
+
+
+def pack_up_adjoint(ct, bn, dev) -> P.PackedConv:
+    """The adjoint of one ConvTranspose2d(k3, s2, p1, op1) + BN stage: a stride-2, zero-border 3x3 contraction with the
+    transposed conv's own weight and the BN scale folded along its input axis."""
+    sc, _ = P.bn_scale_shift(bn)
+    wadj = ct.weight.detach().double() * sc.double()[None, :, None, None]       # [Cin_ct, Cout_ct, 3, 3]
+    return P.pack_conv([(wadj, 0, 0, 1)], None, None, stride=2, border=L.BORDER_ZERO, device=dev)
+
+
+def emit_rear_blocks_backward(prog: Program, saved: list, DX: Buf, sl: Tuple[int, ...], sg: Tuple[int, ...]):
+    """The residual blocks' part of the rear backward, from the bottleneck gradient ``DX`` to the outputs dx0, dx1."""
+    cl, cg = sl[1], sg[1]
     for blk, Y1, Y2 in reversed(saved):
         D1 = emit_ffc_bn_act_backward(prog, blk.conv2, Y2, TV(DX), cl, cg)
         DX = emit_ffc_bn_act_backward(prog, blk.conv1, Y1, TV(D1), cl, cg, extra=TV(DX))

@@ -324,15 +324,23 @@ def build_parser() -> argparse.ArgumentParser:
                     help="refinement: keep the backward's ReLU masks as the forward activations (values, the default) "
                          "or as bits, which needs about half the memory at large scales (same results), e.g. to "
                          "refine 12-24 megapixel photos at full size with a raised --px-budget")
+    ap.add_argument("--refine-tail", choices=("whole", "banded"), default=None,
+                    help="refinement with --relu-masks bits: run the full-resolution up-sampling tail over the whole "
+                         "image (whole, the default) or in row bands with the front run one stage at a time (banded; "
+                         "same results, split-bf16 arithmetic only), e.g. to refine 48-50 megapixel photos at full size "
+                         "on one 80 GB GPU with --px-budget 50000000")
     return ap
 
 
 def refiner_kwargs(a: argparse.Namespace) -> Dict:
-    """Command-line arguments -> lama_b200.refine.BatchedRefiner keyword arguments (``relu_masks`` only when given)."""
+    """Command-line arguments -> lama_b200.refine.BatchedRefiner keyword arguments (``relu_masks`` and ``tail`` only
+    when given)."""
     kw = dict(max_batch=a.batch, modulo=a.pad_mod, n_iters=a.n_iters, lr=a.lr, min_side=a.min_side,
               max_scales=a.max_scales, px_budget=a.px_budget)
     if a.relu_masks is not None:
         kw["relu_masks"] = a.relu_masks
+    if a.refine_tail is not None:
+        kw["tail"] = a.refine_tail
     return kw
 
 

@@ -310,16 +310,35 @@ class BatchedRefiner:
     80 GB GPU.  The results are bit-identical to ``"values"``.  This large-photo setting also keeps one scale's program
     alive at a time (a scale's lane releases the previous one; the batch plan still counts every scale) and releases the
     front's (stem and down-sampling) cached stage programs after each scale's front pass, which at 24 MP would otherwise
-    hold about 34 GB next to the step programs.  Later batches of the same size build and capture them again."""
+    hold about 34 GB next to the step programs.  Later batches of the same size build and capture them again.
+
+    ``tail="banded"`` (with ``relu_masks="bits"`` only) runs the step programs of kind ``generator_refine_bits_banded``:
+    the full-resolution up-sampling tail and head run in row bands (``lama_b200.banded``), which at 24-50 megapixels
+    cuts a step program's storage to less than half the bits program's.  This setting also releases the previous
+    scale's lane before the front (stem and down-sampling) runs, and runs the front's stages one at a time, releasing
+    each stage's programs after it ran, so that 48-50 megapixel photos refine at full size on one 80 GB GPU.
+    The results are bit-identical.  It needs the tensor-core head (split-bf16 arithmetic, ``banded.tail_supported``);
+    the constructor raises ``ValueError`` where that does not hold."""
 
     relu_masks = "values"
+    tail = "whole"
 
     def __init__(self, generator, max_batch: int = 8, *, modulo: int = 8, n_iters: int = 15, lr: float = 0.002,
                  min_side: int = 512, max_scales: int = 3, px_budget: int = 1800000,
-                 mem_budget: Optional[int] = None, relu_masks: str = "values"):
+                 mem_budget: Optional[int] = None, relu_masks: str = "values", tail: str = "whole"):
         if relu_masks not in ("values", "bits"):
             raise ValueError(f"relu_masks must be 'values' or 'bits', not {relu_masks!r}")
-        self.relu_masks = relu_masks
+        if tail not in ("whole", "banded"):
+            raise ValueError(f"tail must be 'whole' or 'banded', not {tail!r}")
+        if tail == "banded" and relu_masks != "bits":
+            raise ValueError("tail='banded' needs relu_masks='bits'")
+        if tail == "banded":
+            from . import engine as E
+            from .banded import tail_supported
+            if not tail_supported(generator, E.default_math()):
+                raise ValueError("tail='banded' needs the tensor-core head: split-bf16 arithmetic (LAMA_B200_MATH), "
+                                 "LAMA_B200_HEAD=tc, a head of at most 3 outputs on a multiple of 8 channels")
+        self.relu_masks, self.tail = relu_masks, tail
         self.generator = generator.eval()
         self.device = next(generator.parameters()).device
         if self.device.type != "cuda":
@@ -384,10 +403,13 @@ class BatchedRefiner:
         return bool(shapes) and all(E.refine_supported(self.generator, sl, sg, crop) for sl, sg, crop in shapes)
 
     def program_kind(self, scale: int, crop: Tuple[int, int]) -> str:
-        """The lowest scale (index 0) runs one forward; every other scale a step program (``relu_masks``: which)."""
+        """The lowest scale (index 0) runs one forward; every other scale a step program (``relu_masks`` and ``tail``:
+        which)."""
         if scale == 0:
             return "generator_rear"
         step = "generator_refine_bits" if self.relu_masks == "bits" else "generator_refine"
+        if self.tail == "banded":
+            step = "generator_refine_bits_banded"
         return f"{step}:{crop[0]}x{crop[1]}"
 
     def per_image_bytes(self, h: int, w: int) -> int:
@@ -421,6 +443,21 @@ class BatchedRefiner:
             self._lanes[key] = lane
         return lane
 
+    def _front_stages(self, x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+        """z1, z2 of the banded setting: the previous scale's lane is released first, then the front's modules run one
+        at a time, each stage's cached programs released right after it ran, so that no more than one stage's buffers
+        are alive (about 68 GB for all of them at 48 megapixels).  The arithmetic is the cached front's."""
+        from . import engine as E
+        self._lanes.clear()
+        torch.cuda.empty_cache()
+        with torch.no_grad():
+            for m in self.front:
+                x = m(x)
+                for sub in m.modules():
+                    E.invalidate(sub)
+                torch.cuda.empty_cache()
+        return x
+
     def _refine_batch(self, images: List[torch.Tensor], masks: List[torch.Tensor]) -> torch.Tensor:
         """Equally sized (1,3,h,w) / (1,1,h,w) CPU images and masks -> (B,3,h',w') refined results on the device."""
         kw, dev = self.kw, self.device
@@ -433,9 +470,14 @@ class BatchedRefiner:
             im = torch.cat([_pad_to_modulo(p[0][s], kw["modulo"]) for p in pyr]).to(dev)
             mk = torch.cat([_pad_to_modulo(p[1][s], kw["modulo"]) for p in pyr]).to(dev)
             mk = (mk >= 1e-8).to(mk.dtype)
-            with torch.no_grad():
-                z1, z2 = self.front(torch.cat([im * (1 - mk), mk], dim=1))
-            if self.relu_masks == "bits":
+            x = torch.cat([im * (1 - mk), mk], dim=1)
+            if self.tail == "banded":
+                z1, z2 = self._front_stages(x)
+            else:
+                with torch.no_grad():
+                    z1, z2 = self.front(x)
+            del x
+            if self.relu_masks == "bits" and self.tail != "banded":
                 # the front's cached stage programs hold full-resolution buffers (about 34 GB for a 24 MP scale); the
                 # large-photo setting releases them before the step program of the scale is built
                 from . import engine as E
