@@ -38,9 +38,9 @@
 extern "C" {
 #endif
 
-#define FFCB_VERSION 115 /* 0.1.5: ffcb_head_bwd7_bits, ffcb_relu_mask_pack_rows, ffcb_relu_bwd_bits_rows,
+#define FFCB_VERSION 116 /* 0.1.6: ffcb_conv_plan (0.1.5: ffcb_head_bwd7_bits, ffcb_relu_mask_pack_rows, ffcb_relu_bwd_bits_rows,
                             ffcb_head_gather7_rows (0.1.4: ffcb_relu_mask_pack, ffcb_relu_bwd_bits; 0.1.3:
-                            ffcb_refine_l1_grad; 0.1.2: ffcb_add, ffcb_head_bwd7; 0.1.1: ffcb_tensor gained cg / tile / sg) */
+                            ffcb_refine_l1_grad; 0.1.2: ffcb_add, ffcb_head_bwd7; 0.1.1: ffcb_tensor gained cg / tile / sg)) */
 
 enum {
   FFCB_OK = 0,
@@ -119,8 +119,13 @@ typedef struct {
  * ring, so the result can feed the next 3x3 reflect contraction without ffcb_fill_reflect_border.  The FP32 arm and
  * every other producer leave the ring to ffcb_fill_reflect_border.
  *
- * weight: FFCB_MATH_FP32  -> float  [Ktot][N]           (N contiguous)
- *         FFCB_MATH_BF16X3 -> bf16  [2][N][Ktot] hi|lo   (K contiguous), Ktot = sum nch
+ * weight: FFCB_MATH_FP32  -> float  [Ktot][N]           (N contiguous), Ktot = sum nch
+ *         FFCB_MATH_BF16X3 -> bf16  [2][N][Kpad] hi|lo   (K contiguous), Kpad = sum of nch rounded up to 64 each,
+ *                                                         the padding columns zero
+ * Reads of the tensor-core arm: it multiplies whole 64-channel blocks, so a segment whose nch is not a multiple of 64
+ * also reads channels [c0 + nch, c0 + 64 * ceil(nch / 64)) of its source that lie inside the view (C) and multiplies
+ * them by the zero padding weights: they must be finite (a NaN or Inf there makes the outputs NaN).  Channels beyond
+ * the view's C and, under FFCB_BORDER_ZERO, everything outside the interior are never read.
  */
 typedef struct {
   ffcb_tensor in[2];
@@ -147,6 +152,31 @@ void ffcb_shutdown(void);
 
 /* Generic fused convolution / pointwise contraction (see ffcb_conv_desc). */
 int ffcb_conv(const ffcb_conv_desc* desc, ffcb_stream_t stream);
+
+/*
+ * Dispatch of the tensor-core arm (FFCB_MATH_BF16X3), from the planning step ffcb_conv itself runs before it encodes
+ * the tensor maps and launches: which kernel instantiation and tiling ffcb_conv would use for `desc` under the current
+ * FFCB_TC_BN / FFCB_TC_ROWS / FFCB_TC_ROWS_TW (read on every call).  Host only: no device call, no tensor map, so it
+ * also answers without a GPU.  A descriptor the arm refuses returns FFCB_EINVAL with the message of ffcb_conv (the
+ * tensor-map encoding at launch can still refuse a descriptor with FFCB_ECUDA).
+ *   kind     FFCB_PLAN_FLAT     dense 1x1 contraction, 128 flattened pixels per M tile
+ *            FFCB_PLAN_SPATIAL  one TMA box per tap and 64-channel block, TW x TH pixel tiles
+ *            FFCB_PLAN_ROWS     rows-resident: one (TH + dy span) x TW halo per M tile, resident weights
+ *            FFCB_PLAN_HALO     column-halo: one (64 ch, TW, TH + 2) box per column shift serves three 3x3 taps
+ *   il, po   tile-blocked A operands / channel-group planar float32 output (template IL / PO)
+ *   ring     the epilogue also writes the output's reflected 1-pixel ring
+ *   bn       N tile (32, 64, 96 or 128); m_tiles x n_tiles tiles over persistent CTAs; stages: pipeline depth
+ */
+enum { FFCB_PLAN_FLAT = 0, FFCB_PLAN_SPATIAL = 1, FFCB_PLAN_ROWS = 2, FFCB_PLAN_HALO = 3 };
+typedef struct {
+  int32_t kind;
+  int32_t il, po, ring;
+  int32_t bn, tw, th, stages;
+  int64_t m_tiles;
+  int32_t n_tiles;
+  int32_t _reserved;
+} ffcb_conv_plan_info;
+int ffcb_conv_plan(const ffcb_conv_desc* desc, ffcb_conv_plan_info* info);
 
 /*
  * Stem: ReflectionPad2d(3) + Conv2d(Cin -> N, k7, no bias) + folded BN + ReLU.

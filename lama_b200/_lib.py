@@ -17,7 +17,8 @@ ACT_NONE, ACT_RELU, ACT_SIGMOID, ACT_TANH = 0, 1, 2, 3
 BORDER_ZERO, BORDER_REFLECT = 0, 1
 MATH_FP32, MATH_BF16X3 = 0, 1
 MAX_KSEG = 64
-VERSION = 115
+PLAN_FLAT, PLAN_SPATIAL, PLAN_ROWS, PLAN_HALO = 0, 1, 2, 3
+VERSION = 116
 
 
 class Tensor(C.Structure):
@@ -41,6 +42,13 @@ class ConvDesc(C.Structure):
                 ("_reserved", C.c_int32), ("seg", KSeg * MAX_KSEG)]
 
 
+class ConvPlanInfo(C.Structure):
+    """``ffcb_conv_plan_info``"""
+    _fields_ = [("kind", C.c_int32), ("il", C.c_int32), ("po", C.c_int32), ("ring", C.c_int32), ("bn", C.c_int32),
+                ("tw", C.c_int32), ("th", C.c_int32), ("stages", C.c_int32), ("m_tiles", C.c_int64),
+                ("n_tiles", C.c_int32), ("_reserved", C.c_int32)]
+
+
 _PT = C.POINTER(Tensor)
 # name -> (restype, argtypes): every symbol include/ffc_b200.h declares
 SIGNATURES = {
@@ -49,6 +57,7 @@ SIGNATURES = {
     "ffcb_check_device": (C.c_int, [C.c_int]),
     "ffcb_shutdown": (None, []),
     "ffcb_conv": (C.c_int, [C.POINTER(ConvDesc), C.c_void_p]),
+    "ffcb_conv_plan": (C.c_int, [C.POINTER(ConvDesc), C.POINTER(ConvPlanInfo)]),
     "ffcb_stem_conv7": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                   _PT, C.c_void_p]),
     "ffcb_stem_pack": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, _PT, C.c_void_p]),

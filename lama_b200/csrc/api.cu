@@ -66,6 +66,7 @@ int check_tensor(const ffcb_tensor* t, const char* name, bool allow_cg) {
 // implemented in the other translation units
 int conv_simt(const ffcb_conv_desc* d, cudaStream_t stream);
 int conv_tc(const ffcb_conv_desc* d, cudaStream_t stream);
+int conv_tc_plan(const ffcb_conv_desc* d, ffcb_conv_plan_info* info);
 int stem_conv7(const float*, int, int, int, int, const float*, const float*, int, const ffcb_tensor*, cudaStream_t);
 int head_conv7(const ffcb_tensor*, const float*, const float*, int, int, float*, cudaStream_t);
 size_t fft2_workspace_bytes(int B, int H, int W, int C);
@@ -162,6 +163,14 @@ int ffcb_conv(const ffcb_conv_desc* d, ffcb_stream_t stream) {
   if (d->math == FFCB_MATH_BF16X3) return conv_tc(d, (cudaStream_t)stream);
   set_error("conv: unknown math mode %d", d->math);
   return FFCB_EINVAL;
+}
+
+int ffcb_conv_plan(const ffcb_conv_desc* d, ffcb_conv_plan_info* info) {
+  int rc = check_conv(d);
+  if (rc) return rc;
+  FFCB_REQUIRE(info != nullptr, "conv_plan: null result");
+  FFCB_REQUIRE(d->math == FFCB_MATH_BF16X3, "conv_plan: only the tensor-core arm (FFCB_MATH_BF16X3) has a plan");
+  return conv_tc_plan(d, info);
 }
 
 int ffcb_stem_conv7(const float* x, int B, int Cin, int H, int W, const float* w, const float* shift, int N,

@@ -710,13 +710,27 @@ int pick_bn(int n) {
   return 128;
 }
 
-}  // namespace
+// Everything a launch needs except the tensor maps, decided on the host from the descriptor (and the FFCB_TC_*
+// variables) alone: conv_tc() launches what plan_tc() decides, ffcb_conv_plan() reports it.
+struct TcPlan {
+  TcParams p;
+  bool used[2], taps[2];
+  int kind;                  // FFCB_PLAN_*
+  bool il, po;               // template parameters IL / PO of the instantiation
+  int rr_span;               // RR: rows of halo below the tile (largest minus smallest dy)
+  int kpad;                  // K of the weight matrix: every segment padded to whole 64-channel blocks
+  int stage_bytes, bar_bytes;
+  size_t smem;
+};
 
-int conv_tc(const ffcb_conv_desc* d, cudaStream_t stream) {
+int plan_tc(const ffcb_conv_desc* d, TcPlan& pl) {
+  TcParams& p = pl.p;
+  bool* used = pl.used;
+  bool* taps = pl.taps;
   // ---- requirements of this arm (the fp32 arm has none of them)
   FFCB_REQUIRE(d->out.B > 0, "conv(tc): empty batch");
   FFCB_REQUIRE((long long)d->out.B * d->out.H * d->out.W < (1ll << 31), "conv(tc): more than 2^31 output pixels");
-  bool used[2] = {false, false}, taps[2] = {false, false};
+  used[0] = used[1] = taps[0] = taps[1] = false;
   int reach[2] = {0, 0};       // furthest tap offset per source: the ring must be at least that wide
   for (int i = 0; i < d->nseg; ++i) {
     used[d->seg[i].src] = true;
@@ -748,7 +762,6 @@ int conv_tc(const ffcb_conv_desc* d, cudaStream_t stream) {
                    s, reach[s]);
   }
 
-  TcParams p;
   p.out = make_view(d->out);
   p.out_planar = d->out.cg != 0 ? 1 : 0;
   p.ring = (d->out.reflect_border && d->out.pad == 1 && d->out.cg == 0 && d->out.fmt == FFCB_BF16X2 && d->out.H >= 4 &&
@@ -793,14 +806,16 @@ int conv_tc(const ffcb_conv_desc* d, cudaStream_t stream) {
   }
   p.flat = flat ? 1 : 0;
   // rows-resident mode (TcParams::rr_*): every segment = the same 64-channel block of one channels-last source, shifted
-  // by dy only (the 7x7 head's row contraction, the windowed 7x7 stem); FFCB_TC_ROWS=0 disables it
+  // by dy only (the 7x7 head's row contraction, the windowed 7x7 stem), into a channels-last output (the RR
+  // instantiation has no planar epilogue), with the resident weights and two halo stages fitting in shared memory;
+  // FFCB_TC_ROWS=0 disables it
   bool rr = false;
-  int rr_dy_min = 0, rr_dy_max = 0;
+  int rr_dy_min = 0, rr_dy_max = 0, rr_tw = 8;
   p.rr_dy0 = p.rr_a_bytes = p.rr_w_bytes = 0;
   {
     const char* e = getenv("FFCB_TC_ROWS");
     rr = !flat && d->stride == 1 && d->nseg >= 3 && p.num_n_tiles == 1 && (e ? atoi(e) != 0 : true) &&
-         d->in[d->seg[0].src].cg == 0;
+         d->in[d->seg[0].src].cg == 0 && d->out.cg == 0;
     rr_dy_min = rr_dy_max = d->seg[0].dy;
     for (int i = 0; i < d->nseg && rr; ++i) {
       const ffcb_kseg& g = d->seg[i];
@@ -810,6 +825,15 @@ int conv_tc(const ffcb_conv_desc* d, cudaStream_t stream) {
       if (g.dy > rr_dy_max) rr_dy_max = g.dy;
     }
     rr = rr && (rr_dy_max - rr_dy_min) <= 8;
+    // a dy shift = TW rows of 128 B must be whole 1024-byte swizzle atoms: TW = 8 (tall tiles: the smallest halo,
+    // 22 rows x 8 pixels = 44 KB per stage for a 7-tap column) or 16; FFCB_TC_ROWS_TW overrides
+    const char* etw = getenv("FFCB_TC_ROWS_TW");
+    rr_tw = (etw && atoi(etw) == 16) ? 16 : 8;
+    if (rr) {
+      const int w_res = d->nseg * 2 * p.BN * BK * 2;
+      const int halo_stage = 2 * (BM / rr_tw + rr_dy_max - rr_dy_min) * rr_tw * BK * 2;
+      rr = (kSmemLimit - 1024 - kBarBytes - w_res) / halo_stage >= 2;
+    }
   }
   // column-halo mode (TcParams::seg_taps): spatial, stride 1, planes wider than 32 (the current tiling's TW >= 64),
   // and channels-last outputs; every segment reads a reflect-ring-padded channels-last source within one pixel
@@ -845,10 +869,7 @@ int conv_tc(const ffcb_conv_desc* d, cudaStream_t stream) {
     p.TW = BM; p.TH = 1; p.tiles_x = p.tiles_y = 1;
     p.num_m_tiles = ((long long)d->out.B * H * W + BM - 1) / BM;
   } else if (rr) {
-    // a dy shift = TW rows of 128 B must be whole 1024-byte swizzle atoms: TW = 8 (tall tiles: the smallest halo,
-    // 22 rows x 8 pixels = 44 KB per stage for a 7-tap column) or 16; FFCB_TC_ROWS_TW overrides
-    const char* etw = getenv("FFCB_TC_ROWS_TW");
-    p.TW = (etw && atoi(etw) == 16) ? 16 : 8;
+    p.TW = rr_tw;
     p.TH = BM / p.TW;
     p.tiles_x = (W + p.TW - 1) / p.TW;
     p.tiles_y = (H + p.TH - 1) / p.TH;
@@ -880,71 +901,104 @@ int conv_tc(const ffcb_conv_desc* d, cudaStream_t stream) {
       FFCB_REQUIRE(p.TW == W && p.TW * p.TH == BM && H % p.TH == 0 && (H * W) % BM == 0,
                    "conv(tc): tile-blocked in[%d] in a spatial contraction needs M tiles of whole rows (W a power of two "
                    "<= 128 dividing 128, H*W a multiple of 128); got %dx%d", s, H, W);
+  // activation coordinates: +pad when the source is mapped with its reflected ring
+  for (int s = 0; s < 2; ++s)
+    p.coord_off[s] = (used[s] && !p.a_il[s] && !flat && taps[s] && d->border == FFCB_BORDER_REFLECT) ? d->in[s].pad : 0;
+  FFCB_REQUIRE(((uintptr_t)d->weight % 16) == 0, "conv(tc): weight pointer not 16-byte aligned");
+  if (d->out.cg == 0) {
+    const ffcb_tensor& t = d->out;
+    const int64_t esz = t.fmt == FFCB_BF16X2 ? 2 : 4;
+    FFCB_REQUIRE(((uintptr_t)t.ptr % 16) == 0 && (t.sx * esz) % 16 == 0 && (t.sy * esz) % 16 == 0 &&
+                     (t.sb * esz) % 16 == 0 && (esz == 4 || (t.lo_off * esz) % 16 == 0),
+                 "conv(tc): out strides / pointer not 16-byte aligned (C must be a multiple of %d)", esz == 2 ? 8 : 4);
+  }
+
+  // stage: RR the halo (hi | lo), HALO one tap's weight tile (hi | lo), else one K block of A and W (hi | lo each);
+  // the resident weights (RR) / the two A buffers (HALO) are carved next to the barriers
+  pl.stage_bytes = rr ? 2 * p.rr_a_bytes : halo ? 2 * p.BN * BK * 2 : 2 * kTileABytes + 2 * p.BN * BK * 2;
+  pl.bar_bytes = kBarBytes + (rr ? p.rr_w_bytes : 0) + (halo ? 4 * p.halo_a_bytes : 0);
+  int stages = (kSmemLimit - 1024 - pl.bar_bytes) / pl.stage_bytes;
+  if (stages > kMaxStages) stages = kMaxStages;
+  FFCB_REQUIRE(stages >= 2, "conv(tc): BN=%d leaves fewer than 2 pipeline stages", p.BN);
+  p.stages = stages;
+  pl.smem = (size_t)stages * pl.stage_bytes + pl.bar_bytes + 1024;
+
+  pl.kind = flat ? FFCB_PLAN_FLAT : rr ? FFCB_PLAN_ROWS : halo ? FFCB_PLAN_HALO : FFCB_PLAN_SPATIAL;
+  pl.il = !rr && !halo && (p.a_il[0] || p.a_il[1]);
+  pl.po = p.out_planar != 0;
+  pl.rr_span = rr ? rr_dy_max - rr_dy_min : 0;
+  pl.kpad = kpad;
+  return FFCB_OK;
+}
+
+}  // namespace
+
+int conv_tc_plan(const ffcb_conv_desc* d, ffcb_conv_plan_info* info) {
+  TcPlan pl;
+  const int rc = plan_tc(d, pl);
+  if (rc) return rc;
+  info->kind = pl.kind;
+  info->il = pl.il;
+  info->po = pl.po;
+  info->ring = pl.p.ring;
+  info->bn = pl.p.BN;
+  info->tw = pl.p.TW;
+  info->th = pl.p.TH;
+  info->stages = pl.p.stages;
+  info->m_tiles = pl.p.num_m_tiles;
+  info->n_tiles = pl.p.num_n_tiles;
+  info->_reserved = 0;
+  return FFCB_OK;
+}
+
+int conv_tc(const ffcb_conv_desc* d, cudaStream_t stream) {
+  TcPlan pl;
+  int rc = plan_tc(d, pl);
+  if (rc) return rc;
+  TcParams& p = pl.p;
+  const bool rr = pl.kind == FFCB_PLAN_ROWS, halo = pl.kind == FFCB_PLAN_HALO, flat = pl.kind == FFCB_PLAN_FLAT;
 
   // ---- tensor maps
   alignas(64) CUtensorMap maps[3];
-  int rc;
   for (int s = 0; s < 2; ++s) {
-    if (!used[s]) { p.coord_off[s] = 0; continue; }     // no tensor map: patched with a valid one below
+    if (!pl.used[s] || p.a_il[s]) continue;     // no tensor map (bulk copies / unused): patched with a valid one below
     const ffcb_tensor& t = d->in[s];
     const cuuint64_t esz = 2;
-    if (p.a_il[s]) { p.coord_off[s] = 0; continue; }       // bulk copies: no tensor map (patched with a valid one below)
     if (flat) {
       cuuint64_t dims[3] = {(cuuint64_t)t.C, (cuuint64_t)t.B * t.H * t.W, 2};
       cuuint64_t str[2] = {(cuuint64_t)t.sx * esz, (cuuint64_t)t.lo_off * esz};
       cuuint32_t box[3] = {BK, BM, 1}, es[3] = {1, 1, 1};
-      p.coord_off[s] = 0;
       if ((rc = encode(&maps[s], t.ptr, 3, dims, str, box, es, "flat activations"))) return rc;
     } else {
-      const bool ring = taps[s] && d->border == FFCB_BORDER_REFLECT;
-      const int off = ring ? t.pad : 0;
+      const int off = p.coord_off[s];
       char* base = (char*)t.ptr - (int64_t)off * ((int64_t)t.sy + t.sx) * (int64_t)esz;
       cuuint64_t dims[5] = {(cuuint64_t)t.C, (cuuint64_t)(t.W + 2 * off), (cuuint64_t)(t.H + 2 * off),
                             (cuuint64_t)t.B, 2};
       cuuint64_t str[4] = {(cuuint64_t)t.sx * esz, (cuuint64_t)t.sy * esz, (cuuint64_t)t.sb * esz,
                            (cuuint64_t)t.lo_off * esz};
       cuuint32_t box[5] = {BK, (cuuint32_t)(p.TW * d->stride), (cuuint32_t)(p.TH * d->stride), 1, 1};
-      if (rr) box[2] = (cuuint32_t)(p.TH + rr_dy_max - rr_dy_min);      // the whole halo of the tile in one box
-      if (halo) box[2] = (cuuint32_t)(p.TH + 2);                         // the tile's rows and one above / below
+      if (rr) box[2] = (cuuint32_t)(p.TH + pl.rr_span);      // the whole halo of the tile in one box
+      if (halo) box[2] = (cuuint32_t)(p.TH + 2);            // the tile's rows and one above / below
       cuuint32_t es[5] = {1, (cuuint32_t)d->stride, (cuuint32_t)d->stride, 1, 1};
-      p.coord_off[s] = off;
       if ((rc = encode(&maps[s], base, 5, dims, str, box, es, "spatial activations"))) return rc;
     }
   }
   {
-    cuuint64_t dims[3] = {(cuuint64_t)kpad, (cuuint64_t)d->n_out, 2};
-    cuuint64_t str[2] = {(cuuint64_t)kpad * 2, (cuuint64_t)kpad * d->n_out * 2};
+    cuuint64_t dims[3] = {(cuuint64_t)pl.kpad, (cuuint64_t)d->n_out, 2};
+    cuuint64_t str[2] = {(cuuint64_t)pl.kpad * 2, (cuuint64_t)pl.kpad * d->n_out * 2};
     cuuint32_t box[3] = {BK, (cuuint32_t)p.BN, 1}, es[3] = {1, 1, 1};
-    FFCB_REQUIRE(((uintptr_t)d->weight % 16) == 0, "conv(tc): weight pointer not 16-byte aligned");
     if ((rc = encode(&maps[2], const_cast<void*>(d->weight), 3, dims, str, box, es, "weights"))) return rc;
   }
-
   for (int s = 0; s < 2; ++s)
-    if (!used[s] || p.a_il[s]) maps[s] = maps[2];      // never dereferenced by the kernel, but prefetched
-  if (d->out.cg == 0) {
-    const ffcb_tensor& t = d->out;
-    const cuuint64_t esz = t.fmt == FFCB_BF16X2 ? 2 : 4;
-    FFCB_REQUIRE(((uintptr_t)t.ptr % 16) == 0 && (t.sx * esz) % 16 == 0 && (t.sy * esz) % 16 == 0 &&
-                     (t.sb * esz) % 16 == 0 && (esz == 4 || (t.lo_off * esz) % 16 == 0),
-                 "conv(tc): out strides / pointer not 16-byte aligned (C must be a multiple of %d)", esz == 2 ? 8 : 4);
-  }
+    if (!pl.used[s] || p.a_il[s]) maps[s] = maps[2];      // never dereferenced by the kernel, but prefetched
 
-  // ---- launch
-  // stage: RR the halo (hi | lo), HALO one tap's weight tile (hi | lo), else one K block of A and W (hi | lo each);
-  // the resident weights (RR) / the two A buffers (HALO) are carved next to the barriers
-  const int stage_bytes = rr ? 2 * p.rr_a_bytes : halo ? 2 * p.BN * BK * 2 : 2 * kTileABytes + 2 * p.BN * BK * 2;
-  const int bar_bytes = kBarBytes + (rr ? p.rr_w_bytes : 0) + (halo ? 4 * p.halo_a_bytes : 0);
-  int stages = (kSmemLimit - 1024 - bar_bytes) / stage_bytes;
-  if (stages > kMaxStages) stages = kMaxStages;
-  FFCB_REQUIRE(stages >= 2, "conv(tc): BN=%d leaves fewer than 2 pipeline stages", p.BN);
-  p.stages = stages;
-  const size_t smem = (size_t)stages * stage_bytes + bar_bytes + 1024;
+  // ---- launch: the instantiation of the plan
   int dev = 0, sms = 132;
   FFCB_CUDA(cudaGetDevice(&dev));
   FFCB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const long long tiles = p.num_m_tiles * p.num_n_tiles;
   const int grid = (int)(tiles < sms ? tiles : sms);
-  const bool any_il = p.a_il[0] || p.a_il[1];
+  const size_t smem = pl.smem;
   auto launch = [&](auto kernel) -> int {
     FFCB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
     kernel<<<grid, kThreads, smem, stream>>>(p, maps[0], maps[1], maps[2]);
@@ -952,13 +1006,13 @@ int conv_tc(const ffcb_conv_desc* d, cudaStream_t stream) {
   };
   auto launch_bn = [&](auto bn) -> int {
     constexpr int N = decltype(bn)::value;
-    if (rr) return launch(conv_tc_kernel<false, false, true, false, N>);
+    if (rr) return launch(conv_tc_kernel<false, false, true, false, N>);      // plan_tc: never il / po
     if (halo) return launch(conv_tc_kernel<false, false, false, true, N>);
-    if (any_il)
-      return p.out_planar ? launch(conv_tc_kernel<true, true, false, false, N>)
-                          : launch(conv_tc_kernel<true, false, false, false, N>);
-    return p.out_planar ? launch(conv_tc_kernel<false, true, false, false, N>)
-                        : launch(conv_tc_kernel<false, false, false, false, N>);
+    if (pl.il)
+      return pl.po ? launch(conv_tc_kernel<true, true, false, false, N>)
+                   : launch(conv_tc_kernel<true, false, false, false, N>);
+    return pl.po ? launch(conv_tc_kernel<false, true, false, false, N>)
+                 : launch(conv_tc_kernel<false, false, false, false, N>);
   };
   switch (p.BN) {
     case 32: rc = launch_bn(std::integral_constant<int, 32>()); break;

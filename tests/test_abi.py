@@ -33,14 +33,17 @@ def test_header_symbols_are_exported_and_bound(lib):
 def test_struct_layouts_match_c(tmp_path):
     from lama_b200 import _lib
     src = tmp_path / "sz.c"
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "ffc_b200.h"\nint main(){printf("%zu %zu %zu %zu %zu\\n",'
-                   'sizeof(ffcb_tensor),sizeof(ffcb_kseg),sizeof(ffcb_conv_desc),offsetof(ffcb_conv_desc,seg),'
-                   'offsetof(ffcb_conv_desc,weight));return 0;}\n')
+    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "ffc_b200.h"\nint main(){printf("%zu %zu %zu %zu %zu '
+                   '%zu %zu %zu\\n",sizeof(ffcb_tensor),sizeof(ffcb_kseg),sizeof(ffcb_conv_desc),offsetof(ffcb_conv_desc,seg),'
+                   'offsetof(ffcb_conv_desc,weight),sizeof(ffcb_conv_plan_info),offsetof(ffcb_conv_plan_info,m_tiles),'
+                   'offsetof(ffcb_conv_plan_info,n_tiles));return 0;}\n')
     exe = tmp_path / "sz"
     subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
-    t, k, d, off_seg, off_w = map(int, subprocess.check_output([str(exe)]).split())
+    t, k, d, off_seg, off_w, p, off_m, off_n = map(int, subprocess.check_output([str(exe)]).split())
     assert ctypes.sizeof(_lib.Tensor) == t and ctypes.sizeof(_lib.KSeg) == k and ctypes.sizeof(_lib.ConvDesc) == d
     assert _lib.ConvDesc.seg.offset == off_seg and _lib.ConvDesc.weight.offset == off_w
+    assert ctypes.sizeof(_lib.ConvPlanInfo) == p
+    assert _lib.ConvPlanInfo.m_tiles.offset == off_m and _lib.ConvPlanInfo.n_tiles.offset == off_n
 
 
 def test_version_and_error_plumbing(lib):
