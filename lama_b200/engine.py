@@ -430,7 +430,7 @@ class Program:
     inputs: Dict[str, Tuple[int, ...]] = field(default_factory=dict)    # name -> NCHW shape
     outputs: Dict[str, Tuple[int, ...]] = field(default_factory=dict)
     dtypes: Dict[str, torch.dtype] = field(default_factory=dict)       # inputs / outputs that are not float32
-    meta: Dict[tuple, dict] = field(default_factory=dict)              # buffers a backward program needs (per module)
+    meta: Dict[tuple, dict] = field(default_factory=dict)              # buffers a backward program needs, ReLU outputs (per module)
     consts: Dict[str, torch.Tensor] = field(default_factory=dict)      # buffer name -> initial contents [B,H,W,C] float
 
     def buf(self, name, B, H, W, C, gemm=False, halo=False, halo_px=1, cg=0) -> Buf:
@@ -819,6 +819,12 @@ def planar_selftest(device: torch.device) -> bool:
     return ok
 
 
+def keep_relu_output(prog: Program, bn, view: TV) -> None:
+    """Record in ``prog.meta`` the view that holds the ReLU output after ``bn`` (keyed by that BN module), so that a
+    test can read the masks the kernels used from the device and pin a float64 reference to them."""
+    prog.meta[("relu", id(bn))] = dict(out=view)
+
+
 def emit_fourier_unit(prog: Program, fu, t: TV, out: TV, residual: Optional[TV]):
     """FourierUnit (ffc.py:76-113): rfft2 -> [1x1 conv + BN + ReLU] on the interleaved spectrum -> irfft2,
     optionally with the SpectralTransform residual fused into the inverse (out = residual + fu(t))."""
@@ -831,6 +837,7 @@ def emit_fourier_unit(prog: Program, fu, t: TV, out: TV, residual: Optional[TV])
     S = prog.buf("spectrum", b, h, wf, cin2, gemm=True, cg=8 if planar else 0)
     Z = prog.buf("spectrum_out", b, h, wf, cout2, cg=8 if planar else 0)
     prog.meta[("fu", id(fu))] = dict(S=S, Z=Z)
+    keep_relu_output(prog, fu.bn, TV(Z))
     scale, shift = P.bn_scale_shift(fu.bn)
     wconv, pos = fu.conv_layer.weight, None
     if fu.spectral_pos_encoding:
@@ -892,6 +899,7 @@ def emit_spectral_transform(prog: Program, st, x: TV, u_consumer=None) -> Tuple[
         tag = "st.conv1+bn+relu"
     prog.ops.append(ConvOp(pk1, [TV(x.buf), None], TV(T), tag=tag))
     prog.meta[("st", id(st))] = dict(T=T, U=U)
+    keep_relu_output(prog, st.conv1[1], TV(T))
     residual = TV(T)
     if st.enable_lfu:
         # xs = lfu(quadrants of the first c/4 channels) tiled 2x2; XS = T + tile(xs) becomes the residual of the main
@@ -938,6 +946,10 @@ def emit_ffc_bn_act(prog: Program, m, X: Buf, in_cl: int, in_cg: int, residual: 
     has_spectral = not isinstance(f.convg2g, nn.Identity)
     res_l = TV(residual, 0, out_cl) if residual is not None else None
     res_g = TV(residual, out_cl, out_cg) if residual is not None else None
+    if residual is None:            # Y holds the activations themselves
+        for bn, act, c0, n in ((m.bn_l, act_l, 0, out_cl), (m.bn_g, act_g, out_cl, out_cg)):
+            if n > 0 and act == L.ACT_RELU:
+                keep_relu_output(prog, bn, TV(Y, c0, n))
 
     if in_cg == 0 and out_cl > 0 and out_cg > 0 and act_l == act_g:
         # local input only (stem-like / downsample-to-global): convl2l and convl2g read the same
@@ -993,7 +1005,9 @@ def emit_resnet_block(prog: Program, blk, X: Buf, cl: int, cg: int, in_place: bo
 # for: every plane the native FFT pair takes.  Its input gradients are tested against float64 autograd through the
 # oracle from 12x20 up to 256x256 (tests/test_gpu_parity.py, tests/test_gpu_program_diff.py), at 211x251 (Bluestein,
 # tests/test_gpu_fft_bluestein.py) and at 270x480, 259x108 and 128x1024 (8-channel and Bluestein FFT lengths,
-# tests/test_gpu_refine_large_planes.py).  Wider planes are rejected by the FFT kernels and take torch autograd.
+# tests/test_gpu_refine_large_planes.py), and at all of these element by element against float64 autograd run with the
+# kernels' own ReLU masks (tests/test_gpu_pinned_grads.py).  Wider planes are rejected by the FFT kernels and take
+# torch autograd.
 BLOCK_GRAD_MAX_PLANE = FFT_MAX_LEN
 
 
@@ -1304,6 +1318,7 @@ def emit_up_tail(prog: Program, ups, X: Buf, tc_head: bool) -> List[Buf]:
         for a, bb, pk in P.pack_conv_transpose_phases(ct.weight, ct.bias, sc, sh, act=L.ACT_RELU,
                                                       device=ct.weight.device):
             prog.ops.append(ConvOp(pk, [TV(X), None], TV(Yb, phase=(a, bb)), tag=f"convT phase {a}{bb}+bn+relu"))
+        keep_relu_output(prog, bn, TV(Yb))
         X = Yb
         outs.append(Yb)
     return outs

@@ -13,10 +13,60 @@ Never imported by the product path (``lama_b200``).
 """
 from __future__ import annotations
 
+import contextlib
+
 import torch
 import torch.nn.functional as F
 
 EPS = 1e-5
+
+# Pinned ReLU masks (``pinned_relu_masks``): None, or (site -> mask, set of the sites served)
+_PINNED = None
+# Masks recorded by ``recorded_relu_masks``: None, or site -> mask
+_RECORDED = None
+
+
+def relu(x, site):
+    """The ReLU (in place) after the eval-mode BN whose state-dict prefix is ``site`` (``...bn_l.``, ``...bn_g.``,
+    ``...convg2g.conv1.1.``, ``...fu.bn.``, ``model.{i}.`` of an up stage).  Under ``pinned_relu_masks`` it is
+    ``x * mask[site]``: linear in x, with the mask given instead of the one x implies."""
+    if _PINNED is None:
+        y = torch.relu_(x)
+        if _RECORDED is not None:
+            _RECORDED[site] = (y > 0).detach()
+        return y
+    masks, served = _PINNED
+    if site not in masks:
+        raise KeyError(f"no pinned ReLU mask for site {site!r}")
+    if tuple(masks[site].shape) != tuple(x.shape):
+        raise ValueError(f"the pinned ReLU mask of {site!r} is {tuple(masks[site].shape)}, its input {tuple(x.shape)}")
+    served.add(site)
+    return x * masks[site]
+
+
+@contextlib.contextmanager
+def recorded_relu_masks():
+    """Yield a dict that collects, per site, the mask (output > 0) of every ReLU evaluated inside without pinned masks."""
+    global _RECORDED
+    prev, _RECORDED = _RECORDED, {}
+    try:
+        yield _RECORDED
+    finally:
+        _RECORDED = prev
+
+
+@contextlib.contextmanager
+def pinned_relu_masks(masks):
+    """Evaluate every ReLU of the functions below as ``x * masks[site]`` (masks: bool or 0 / 1, of x's NCHW shape).  A
+    gradient program is linear once its masks are fixed, so with the masks a device run used, autograd through this
+    module differs from that run by round-off alone.  Yields the set of sites served; a site without a mask raises."""
+    global _PINNED
+    served = set()
+    prev, _PINNED = _PINNED, (dict(masks), served)
+    try:
+        yield served
+    finally:
+        _PINNED = prev
 
 
 def _bn(x, sd, p):
@@ -38,7 +88,7 @@ def fourier_unit(x, sd, p=""):
     f = torch.fft.rfftn(x, dim=(-2, -1), norm="ortho")                         # :86
     f = torch.stack((f.real, f.imag), dim=-1).permute(0, 1, 4, 2, 3).contiguous()   # :87-88
     f = f.view((b, -1) + tuple(f.shape[3:]))                                   # :89
-    f = torch.relu_(_bn(F.conv2d(f, sd[p + "conv_layer.weight"]), sd, p + "bn."))   # :100-101
+    f = relu(_bn(F.conv2d(f, sd[p + "conv_layer.weight"]), sd, p + "bn."), p + "bn.")   # :100-101
     f = f.view((b, -1, 2) + tuple(f.shape[2:])).permute(0, 1, 3, 4, 2).contiguous()  # :103-104
     f = torch.complex(f[..., 0], f[..., 1])                                    # :105
     return torch.fft.irfftn(f, s=x.shape[-2:], dim=(-2, -1), norm="ortho")      # :108
@@ -48,7 +98,7 @@ def spectral_transform(x, sd, p="", stride=1, enable_lfu=False):
     """ffc.py:142-163."""
     if stride == 2:
         x = F.avg_pool2d(x, 2, 2)
-    x = torch.relu_(_bn(F.conv2d(x, sd[p + "conv1.0.weight"]), sd, p + "conv1.1."))
+    x = relu(_bn(F.conv2d(x, sd[p + "conv1.0.weight"]), sd, p + "conv1.1."), p + "conv1.1.")
     out = fourier_unit(x, sd, p + "fu.")
     if enable_lfu:
         n, c, h, w = x.shape
@@ -70,12 +120,12 @@ def ffc_bn_act(x_l, x_g, sd, p, *, ratio_gout, stride=1, padding=0, dilation=1, 
         o_l = _conv(x_l, sd[q + "convl2l.weight"], **kw)
         if (q + "convg2l.weight") in sd:
             o_l = o_l + _conv(x_g, sd[q + "convg2l.weight"], **kw)
-        o_l = torch.relu_(_bn(o_l, sd, p + "bn_l."))
+        o_l = relu(_bn(o_l, sd, p + "bn_l."), p + "bn_l.")
     if ratio_gout != 0:
         o_g = _conv(x_l, sd[q + "convl2g.weight"], **kw)
         if (q + "convg2g.conv2.weight") in sd:
             o_g = o_g + spectral_transform(x_g, sd, q + "convg2g.", stride=stride, enable_lfu=enable_lfu)
-        o_g = torch.relu_(_bn(o_g, sd, p + "bn_g."))
+        o_g = relu(_bn(o_g, sd, p + "bn_g."), p + "bn_g.")
     return o_l, o_g
 
 
@@ -99,7 +149,7 @@ def generator_rear(z1, z2, sd, kw):
     for _ in range(nd):
         h = F.conv_transpose2d(h, sd[f"model.{i}.weight"], sd[f"model.{i}.bias"], stride=2, padding=1,
                                output_padding=1)
-        h = torch.relu(_bn(h, sd, f"model.{i + 1}.")); i += 3
+        h = relu(_bn(h, sd, f"model.{i + 1}."), f"model.{i + 1}."); i += 3
     h = F.conv2d(F.pad(h, (3, 3, 3, 3), mode="reflect"), sd[f"model.{i + 1}.weight"], sd[f"model.{i + 1}.bias"])
     act = kw.get("add_out_act", True)
     if act is True or act == "tanh":
@@ -130,7 +180,7 @@ def ffc_resnet_generator(x, sd, *, ngf=64, n_downsampling=3, n_blocks=9, init_co
     for _ in range(n_downsampling):
         h = F.conv_transpose2d(h, sd[f"{prefix}{i}.weight"], sd[f"{prefix}{i}.bias"], stride=2, padding=1,
                                output_padding=1); i += 1
-        h = torch.relu_(_bn(h, sd, f"{prefix}{i}.")); i += 2
+        h = relu(_bn(h, sd, f"{prefix}{i}."), f"{prefix}{i}."); i += 2
     h = F.pad(h, (3, 3, 3, 3), mode="reflect"); i += 1
     h = F.conv2d(h, sd[f"{prefix}{i}.weight"], sd[f"{prefix}{i}.bias"]); i += 1
     if add_out_act:

@@ -1,6 +1,6 @@
 """Block, layer and generator programs on the GPU at bottleneck planes wider than 64 pixels.
 
-1. Op by op (``diff_program``): one ``engine.Program`` is issued through ``CudaExecutor`` one C-ABI call at a time.
+1. Op by op (``device_state.diff_program``): one ``engine.Program`` is issued through ``CudaExecutor`` one C-ABI call at a time.
    Before each call the device buffers the op touches are decoded to float64 and loaded into ``SpecInterpreter``; after
    the call the interpreter runs that op alone and every view the op wrote is compared with what the kernel wrote.
    Each op is judged on the device state it actually saw (its buffers, and the program outputs written so far), so
@@ -26,9 +26,8 @@ from lama_b200 import modules as M                   # noqa: E402
 from lama_b200.testing import seeded_parameters_, small_lama_kwargs  # noqa: E402
 from oracle import ffc_numpy as onp                  # noqa: E402
 from oracle import ffc_torch_cpu as otc              # noqa: E402
-from spec_interp import SpecInterpreter              # noqa: E402
+from device_state import DEV, diff_program           # noqa: E402
 
-DEV = "cuda:0"
 MATHS = {"fp32": L.MATH_FP32, "bf16x3": L.MATH_BF16X3}
 TOL = {"fp32": 2e-5, "bf16x3": 2e-4}                 # module level, as in test_gpu_parity.py
 
@@ -51,153 +50,6 @@ def math_mode(request):
     os.environ["LAMA_B200_MATH"] = request.param
     yield request.param
     os.environ.pop("LAMA_B200_MATH", None)
-
-
-# ------------------------------------------------------------------------------------------- decoding
-class Decoder:
-    """Device storage of a ``Buf`` -> float64 [B, H, W, C] on the CPU, addressed as include/ffc_b200.h defines it
-    (independent of the shape the executor allocated the storage with):
-      plain             (b, y, x, c) at ((b*Hp + y+p)*Wp + x+p)*C + c      (Hp, Wp: with the ring of p pixels)
-      channel groups    (b, y, x, c) at (c/cg)*B*H*W*cg + ((b*H + y)*W + x)*cg + c%cg
-      tile-blocked      (m, c) at (m/128)*sg + (c/8)*1024 + (m%128)*8 + c%8,  m = (b*H + y)*W + x, sg = C/8*1024
-    Split bf16 is hi + lo with the lo plane ``lo_off`` elements after the hi plane."""
-
-    def __init__(self, ex):
-        self.ex = ex
-        self._idx = {}
-
-    def _index(self, b):
-        if b.name not in self._idx:
-            p = b.pad
-            B, H, W, C = b.B, b.H + 2 * p, b.W + 2 * p, b.C
-            ar = lambda n, d: torch.arange(n, device=DEV).view([-1 if i == d else 1 for i in range(4)])  # noqa: E731
-            bi, y, x, c = ar(B, 0), ar(H, 1), ar(W, 2), ar(C, 3)
-            if b.tile:
-                assert b.cg == 8 and b.tile == 128 and p == 0
-                m = (bi * H + y) * W + x
-                idx = (m // 128) * (C // 8 * 1024) + (c // 8) * 1024 + (m % 128) * 8 + c % 8
-                lo_off = -(-(B * H * W) // 128) * (C // 8) * 1024
-            elif b.cg:
-                assert p == 0
-                idx = (c // b.cg) * (B * H * W * b.cg) + ((bi * H + y) * W + x) * b.cg + c % b.cg
-                lo_off = B * H * W * C
-            else:
-                idx = ((bi * H + y) * W + x) * C + c
-                lo_off = B * H * W * C
-            self._idx[b.name] = (idx, lo_off)
-        return self._idx[b.name]
-
-    def __call__(self, b, ring=False):
-        """Interior [B, H, W, C]; with ``ring`` the whole padded plane [B, H+2p, W+2p, C]."""
-        idx, lo_off = self._index(b)
-        flat = self.ex.storage[b.name].reshape(-1)
-        if b.fmt == L.F32:
-            v = flat[idx].double()
-        else:
-            v = flat[idx].double() + flat[idx + lo_off].double()
-        if b.pad and not ring:
-            p = b.pad
-            v = v[:, p:p + b.H, p:p + b.W]
-        return v.cpu()
-
-
-def split_bf16(v: torch.Tensor) -> torch.Tensor:
-    """The value a split-bf16 store keeps of ``v``: hi = bf16(v), lo = bf16(v - hi), in float32 (csrc/common.cuh)."""
-    f = v.float()
-    hi = f.bfloat16().float()
-    return hi.double() + (f - hi).bfloat16().double()
-
-
-def ring_is_reflection(full: torch.Tensor, p: int) -> bool:
-    """[B, H+2p, W+2p, C]: does every ring pixel hold the reflection (no edge repeat) of the interior?"""
-    h, w = full.shape[1] - 2 * p, full.shape[2] - 2 * p
-
-    def refl(n):
-        i = (torch.arange(-p, n + p)).abs()
-        return torch.where(i >= n, 2 * n - 2 - i, i)
-    want = full[:, p:p + h, p:p + w][:, refl(h)][:, :, refl(w)]
-    return torch.equal(full, want)
-
-
-# ------------------------------------------------------------------------------------------- per-op check
-def op_label(i, op) -> str:
-    s = f"op {i} {type(op).__name__}"
-    if isinstance(op, E.ConvOp):
-        s += f" [{op.tag}]"
-    _, writes = op.views()
-    return s + "".join(f" -> {tv.buf.name}" for tv in writes)
-
-
-def op_tol(op, math: int, out_fmt: int):
-    """(limit on max-abs / max|ref|, compare against the split-bf16 rounding of the reference?)"""
-    if isinstance(op, (E.ConvOp, E.StemOp, E.HeadOp, E.HeadGatherOp, E.HeadBwdOp)):           # contractions
-        return (2e-4 if math == L.MATH_BF16X3 else 2e-5), False
-    if isinstance(op, (E.RfftOp, E.IrfftOp)):
-        return (2e-5 if out_fmt == L.BF16X2 else 2e-6), False
-    return 1e-6, out_fmt == L.BF16X2           # layout, ring, ReLU backward, fold, add, loss: exact up to the storage format
-
-
-def _rel(got, ref) -> float:
-    scale = float(ref.abs().max()) if ref.numel() else 0.0
-    return float((got - ref).abs().max()) / (scale or 1.0) if ref.numel() else 0.0
-
-
-def diff_program(prog: E.Program, inputs, after_call=None):
-    """Run ``prog`` on the GPU one call at a time and judge every op against the interpreter, fed with the device
-    state the kernel saw.  ``after_call(i, op, ex)`` runs right after the call of op i (the harness self-test uses it).
-    Returns [(op index, label, error, limit)] of the ops that disagree, and raises on a bad reflected ring."""
-    ex = E.CudaExecutor(prog, torch.device(DEV))
-    assert len(ex.calls) == sum(not isinstance(op, E.SplitOp) for op in prog.ops)
-    feed = {k: v.to(DEV).contiguous() for k, v in inputs.items()}
-    ex.bind_inputs(feed)
-    host_in = {k: v.cpu() for k, v in inputs.items()}
-    dec = Decoder(ex)
-    interp = SpecInterpreter(prog)
-    stream = torch.cuda.current_stream().cuda_stream
-    calls = iter(ex.calls)
-    bad = []
-    torch.cuda.synchronize()
-    for i, op in enumerate(prog.ops):
-        if isinstance(op, E.SplitOp):
-            continue
-        reads, writes = op.views()
-        touched = {tv.buf.name: tv.buf for tv in reads + writes}
-        for name, b in touched.items():
-            interp.mem[name] = dec(b)
-        if isinstance(op, E.ConvOp) and op.packed.border == L.BORDER_REFLECT:
-            for s, tv in enumerate(op.ins):
-                if tv is not None and tv.buf.pad and any(g.src == s and (g.dy or g.dx) for g in op.packed.segs):
-                    assert ring_is_reflection(dec(tv.buf, ring=True), tv.buf.pad), \
-                        f"{op_label(i, op)}: the ring of input {tv.buf.name} is not the reflection of its interior"
-        name, fn, args = next(calls)
-        L.check(fn(*args, stream), name)
-        if after_call is not None:
-            after_call(i, op, ex)
-        torch.cuda.synchronize()
-        out = {k: v.cpu() for k, v in ex.outputs.items()}     # the device's outputs as they stand before the call
-        before = dict(out)
-        interp.step(op, host_in, out)
-        worst = None
-        for tv in writes:
-            ref = interp.read(tv)
-            want = interp.mem[tv.buf.name]
-            interp.mem[tv.buf.name] = dec(tv.buf)
-            got = interp.read(tv)
-            interp.mem[tv.buf.name] = want
-            tol, rounded = op_tol(op, prog.math, tv.buf.fmt)
-            err = _rel(got, split_bf16(ref) if rounded else ref)
-            if not err <= tol:
-                worst = (i, op_label(i, op), err, tol)
-        for dst in prog.outputs:
-            if out[dst] is before[dst]:
-                continue                                # not written by this op
-            tol, _ = op_tol(op, prog.math, L.F32)
-            err = _rel(ex.outputs[dst].cpu().double(), out[dst].double())
-            if not err <= tol:
-                worst = (i, op_label(i, op) + f" -> {dst}", err, tol)
-        if worst is not None:
-            bad.append(worst)
-    return bad
 
 
 def _block(dim, seed=4):

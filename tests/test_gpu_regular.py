@@ -1,6 +1,6 @@
 """LaMa-Regular generators (``lama_b200.pix2pixhd.GlobalGenerator``: lama-regular, big-lama-regular) on the GPU.
 
-1. Op by op (``diff_program`` of test_gpu_program_diff.py): every op of the small (ngf 8) program, float and uint8
+1. Op by op (``diff_program`` of device_state.py): every op of the small (ngf 8) program, float and uint8
    variants, and of a program with lama-regular's widths at 64x64 and 48x80 bottleneck planes is judged on the device
    state it read.  This covers the two contractions these models add to ``conv_tc_kernel``: the 512 -> 512 3x3
    reflect contraction in column-halo mode with four N tiles, and the 3x3 stride-2 zero-border contraction as a
@@ -24,7 +24,7 @@ from lama_b200 import engine as E                    # noqa: E402
 from lama_b200 import pix2pixhd as PX                # noqa: E402
 from lama_b200.testing import (LAMA_REGULAR_KWARGS, generator_input, seeded_parameters_,  # noqa: E402
                                small_regular_kwargs, synthetic_image_mask)
-from test_gpu_program_diff import diff_program       # noqa: E402
+from device_state import diff_program                # noqa: E402
 
 DEV = "cuda:0"
 MATHS = {"fp32": L.MATH_FP32, "bf16x3": L.MATH_BF16X3}
