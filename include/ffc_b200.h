@@ -38,7 +38,7 @@
 extern "C" {
 #endif
 
-#define FFCB_VERSION 116 /* 0.1.6: ffcb_conv_plan (0.1.5: ffcb_head_bwd7_bits, ffcb_relu_mask_pack_rows, ffcb_relu_bwd_bits_rows,
+#define FFCB_VERSION 117 /* 0.1.7: ffcb_stem_bwd7 (0.1.6: ffcb_conv_plan; 0.1.5: ffcb_head_bwd7_bits, ffcb_relu_mask_pack_rows, ffcb_relu_bwd_bits_rows,
                             ffcb_head_gather7_rows (0.1.4: ffcb_relu_mask_pack, ffcb_relu_bwd_bits; 0.1.3:
                             ffcb_refine_l1_grad; 0.1.2: ffcb_add, ffcb_head_bwd7; 0.1.1: ffcb_tensor gained cg / tile / sg)) */
 
@@ -343,6 +343,19 @@ int ffcb_head_bwd7_bits(const float* y_nchw, const float* dy_nchw, int B, int N,
                         const uint32_t* mask_bits, int row0, const ffcb_tensor* out, ffcb_stream_t stream);
 int ffcb_head_gather7_rows(const ffcb_tensor* q, const float* bias, int N, int act, float* y_nchw, int H, int row0,
                            ffcb_stream_t stream);
+
+/*
+ * Input gradient through the whole generator (lama_b200/generator_grad.py): the adjoint of the stem's
+ * ReflectionPad2d(3) -> Conv2d(Cin -> N, k7) (ffc.py:314-316, pix2pixhd.py:365-366) w.r.t. the NCHW input:
+ *   ffcb_stem_bwd7: dx = Fold3(Conv7^T(g))
+ *                   g: (B, H, W, N) view of the gradient w.r.t. the stem's pre-activation (its ReLU mask applied),
+ *                   either storage format, any ring; w: float [N][7*7][Cin] (the stem weight with the BN scale
+ *                   folded along N); dx: float NCHW [B][Cin][H][W], overwritten.  Conv7^T scatters every pixel's
+ *                   gradient over its 7x7 window of the (H+6)x(W+6) padded plane, Fold3 adds each padded position onto
+ *                   the interior pixel the reflection copied it from.  1 <= Cin <= 16, H, W >= 4.  No atomics: each
+ *                   pixel sums its terms in one order, independent of the batch and the tiling.
+ */
+int ffcb_stem_bwd7(const ffcb_tensor* g, const float* w, int Cin, float* dx_nchw, ffcb_stream_t stream);
 
 /*
  * Gradient of the refinement loss w.r.t. the prediction (evaluation/refinement.py:75-84 _l1_loss, 19-26 _pyrdown,

@@ -18,7 +18,7 @@ BORDER_ZERO, BORDER_REFLECT = 0, 1
 MATH_FP32, MATH_BF16X3 = 0, 1
 MAX_KSEG = 64
 PLAN_FLAT, PLAN_SPATIAL, PLAN_ROWS, PLAN_HALO = 0, 1, 2, 3
-VERSION = 116
+VERSION = 117
 
 
 class Tensor(C.Structure):
@@ -85,6 +85,7 @@ SIGNATURES = {
     "ffcb_relu_bwd_bits_rows": (C.c_int, [_PT, C.c_void_p, C.c_int, C.c_int, _PT, C.c_void_p]),
     "ffcb_head_gather7_rows": (C.c_int, [_PT, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int,
                                          C.c_void_p]),
+    "ffcb_stem_bwd7": (C.c_int, [_PT, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "ffcb_refine_l1_grad": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p] + [C.c_int] * 6 + [C.c_void_p] * 7
                             + [C.c_void_p]),
     "ffcb_launch_count": (C.c_longlong, []),

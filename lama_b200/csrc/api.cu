@@ -93,6 +93,7 @@ int head_bwd7(const float*, const float*, int, int, int, int, const float*, int,
               cudaStream_t);
 int head_bwd7_bits(const float*, const float*, int, int, int, int, const float*, int, const uint32_t*, int,
                    const ffcb_tensor*, cudaStream_t);
+int stem_bwd7(const ffcb_tensor*, const float*, int, float*, cudaStream_t);
 int refine_l1_grad(const float*, const float*, const float*, int, int, int, int, int, int, const float*, const float*,
                    const float*, const float*, float*, float*, float*, cudaStream_t);
 
@@ -248,6 +249,10 @@ int ffcb_add(const ffcb_tensor* a, const ffcb_tensor* b, const ffcb_tensor* out,
 int ffcb_head_bwd7(const float* y_nchw, const float* dy_nchw, int B, int N, int H, int W, const float* w, int act,
                    const ffcb_tensor* mask, const ffcb_tensor* out, ffcb_stream_t stream) {
   return head_bwd7(y_nchw, dy_nchw, B, N, H, W, w, act, mask, out, (cudaStream_t)stream);
+}
+
+int ffcb_stem_bwd7(const ffcb_tensor* g, const float* w, int Cin, float* dx_nchw, ffcb_stream_t stream) {
+  return stem_bwd7(g, w, Cin, dx_nchw, (cudaStream_t)stream);
 }
 
 int ffcb_head_bwd7_bits(const float* y_nchw, const float* dy_nchw, int B, int N, int H, int W, const float* w,

@@ -279,7 +279,136 @@ __global__ void __launch_bounds__(HB_THREADS) head_bwd7_kernel(const float* __re
   }
 }
 
+// ---- stem backward: dx = Fold3(Conv7^T(g)) ------------------------------------------------------------------------
+// The adjoint of ReflectionPad2d(3) + the 7x7 stem conv (ffc.py:314-316, pix2pixhd.py:365-366) w.r.t. the generator's
+// NCHW input.  Cin <= 16 outputs over K = N*49 is far too narrow for wgmma, so it runs on CUDA cores in the structure
+// of head_bwd7_kernel: one CTA holds SB_TH x SB_TW interior pixels of one image, every Cin; per chunk of SB_NC gradient
+// channels it stages g over the tile plus a 3-pixel apron (zero outside the plane) and that chunk's weights in shared
+// memory.  A thread owns 2 pixels 16 columns apart, all CP (Cin rounded up to 4, 8 or 16) outputs.  The reflected
+// terms (padded rows 3-y and 2H+1-y, columns likewise) exist for pixels within 4 of an edge and run per pixel, from
+// the same shared tile (see head_bwd7_kernel for why they never leave it).  Each pixel's sum runs in one fixed order
+// — per chunk the main term over (ky, kx, n), then its reflected terms — whatever the tile or the batch.
+constexpr int SB_TH = 16, SB_TW = 32, SB_GR = SB_TH + 6, SB_GC = SB_TW + 6, SB_THREADS = 256;
+
+template <int CP, int NC>
+__global__ void __launch_bounds__(SB_THREADS) stem_bwd7_kernel(View g, const float* __restrict__ w, int Cin,
+                                                                float* __restrict__ dx) {
+  __shared__ float g_s[NC][SB_GR][SB_GC];
+  __shared__ __align__(16) float w_s[49 * NC * CP];      // [tap][n][c]
+  const int H = g.H, W = g.W, N = g.C;
+  const int b = blockIdx.z, y0 = blockIdx.y * SB_TH, x0 = blockIdx.x * SB_TW;
+  const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
+  const int yy = y0 + ty;
+  float acc[2][CP];
+#pragma unroll
+  for (int j = 0; j < 2; ++j)
+#pragma unroll
+    for (int c = 0; c < CP; ++c) acc[j][c] = 0.f;
+  // padded rows / columns ReflectionPad2d(3) copied from each owned pixel: the main one first
+  int rows[3], nr = 1;
+  rows[0] = yy + 3;
+  if (yy >= 1 && yy <= 3) rows[nr++] = 3 - yy;
+  if (yy >= H - 4 && yy <= H - 2) rows[nr++] = 2 * H + 1 - yy;
+  for (int n0 = 0; n0 < N; n0 += NC) {
+    const int nc = min(NC, N - n0);
+    __syncthreads();
+    for (int i = tid; i < 49 * NC * CP; i += SB_THREADS) {       // w: [N][49][Cin] -> [49][NC][CP], zero-padded
+      const int c = i % CP, nl = (i / CP) % NC, tap = i / (CP * NC);
+      w_s[i] = (c < Cin && nl < nc) ? w[((long long)(n0 + nl) * 49 + tap) * Cin + c] : 0.f;
+    }
+    for (int i = tid; i < NC * SB_GR * SB_GC; i += SB_THREADS) {  // channels fastest: runs of NC channels per pixel
+      const int nl = i % NC, cx = (i / NC) % SB_GC, r = i / (NC * SB_GC);
+      const int oy = y0 - 3 + r, ox = x0 - 3 + cx;
+      float v = 0.f;
+      if (nl < nc && oy >= 0 && oy < H && ox >= 0 && ox < W) v = load1(g, pix_off(g, b, oy, ox) + n0 + nl);
+      g_s[nl][r][cx] = v;
+    }
+    __syncthreads();
+    // main term: padded position (y+3, x+3) receives g[y+3-ky][x+3-kx] w[ky][kx], local row ty + 6 - ky
+#pragma unroll 1
+    for (int ky = 0; ky < 7; ++ky)
+#pragma unroll 1
+      for (int kx = 0; kx < 7; ++kx)
+#pragma unroll 2
+        for (int nl = 0; nl < NC; ++nl) {
+          const float ga = g_s[nl][ty + 6 - ky][tx + 6 - kx], gb = g_s[nl][ty + 6 - ky][tx + 22 - kx];
+          const float4* wr = reinterpret_cast<const float4*>(w_s + ((ky * 7 + kx) * NC + nl) * CP);
+#pragma unroll
+          for (int q = 0; q < CP / 4; ++q) {
+            const float4 wv = wr[q];
+            acc[0][4 * q] = __fmaf_rn(ga, wv.x, acc[0][4 * q]);
+            acc[0][4 * q + 1] = __fmaf_rn(ga, wv.y, acc[0][4 * q + 1]);
+            acc[0][4 * q + 2] = __fmaf_rn(ga, wv.z, acc[0][4 * q + 2]);
+            acc[0][4 * q + 3] = __fmaf_rn(ga, wv.w, acc[0][4 * q + 3]);
+            acc[1][4 * q] = __fmaf_rn(gb, wv.x, acc[1][4 * q]);
+            acc[1][4 * q + 1] = __fmaf_rn(gb, wv.y, acc[1][4 * q + 1]);
+            acc[1][4 * q + 2] = __fmaf_rn(gb, wv.z, acc[1][4 * q + 2]);
+            acc[1][4 * q + 3] = __fmaf_rn(gb, wv.w, acc[1][4 * q + 3]);
+          }
+        }
+    if (yy >= H) continue;
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const int xx = x0 + tx + 16 * j;
+      if (xx >= W) continue;
+      int cols[3], ncol = 1;
+      cols[0] = xx + 3;
+      if (xx >= 1 && xx <= 3) cols[ncol++] = 3 - xx;
+      if (xx >= W - 4 && xx <= W - 2) cols[ncol++] = 2 * W + 1 - xx;
+      if (nr == 1 && ncol == 1) continue;
+      for (int a = 0; a < nr; ++a)
+        for (int e = 0; e < ncol; ++e) {
+          if (a == 0 && e == 0) continue;                          // the main term, done above
+          for (int ky = 0; ky < 7; ++ky) {
+            const int lr = rows[a] - ky - y0 + 3;                  // local row of g[py - ky]
+            if (lr < 0 || lr >= SB_GR) continue;
+            for (int kx = 0; kx < 7; ++kx) {
+              const int lc = cols[e] - kx - x0 + 3;
+              if (lc < 0 || lc >= SB_GC) continue;
+              for (int nl = 0; nl < NC; ++nl) {
+                const float gv = g_s[nl][lr][lc];
+                const float* wr = w_s + ((ky * 7 + kx) * NC + nl) * CP;
+#pragma unroll
+                for (int c = 0; c < CP; ++c) acc[j][c] = __fmaf_rn(gv, wr[c], acc[j][c]);
+              }
+            }
+          }
+        }
+    }
+  }
+  if (yy >= H) return;
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const int xx = x0 + tx + 16 * j;
+    if (xx >= W) continue;
+#pragma unroll
+    for (int c = 0; c < CP; ++c)
+      if (c < Cin) dx[(((long long)b * Cin + c) * H + yy) * W + xx] = acc[j][c];
+  }
+}
+
 }  // namespace
+
+int stem_bwd7(const ffcb_tensor* g, const float* w, int Cin, float* dx, cudaStream_t stream) {
+  int rc;
+  if ((rc = check_tensor(g, "stem_bwd7.g"))) return rc;
+  FFCB_REQUIRE(Cin >= 1 && Cin <= 16, "stem_bwd7: Cin=%d outside [1,16]", Cin);
+  FFCB_REQUIRE(g->H >= 4 && g->W >= 4, "stem_bwd7: ReflectionPad2d(3) needs H, W >= 4 (got %dx%d)", g->H, g->W);
+  FFCB_REQUIRE(!g->window, "stem_bwd7: window views are not accepted");
+  FFCB_REQUIRE(w != nullptr && dx != nullptr, "stem_bwd7: null pointer");
+  if ((long long)g->B * g->H * g->W * g->C == 0) return FFCB_OK;
+  FFCB_REQUIRE(g->B <= 65535, "stem_bwd7: batch %d too large", g->B);
+  dim3 grid((g->W + SB_TW - 1) / SB_TW, (g->H + SB_TH - 1) / SB_TH, g->B);
+  const View v = make_view(*g);
+  if (Cin <= 4)
+    stem_bwd7_kernel<4, 8><<<grid, SB_THREADS, 0, stream>>>(v, w, Cin, dx);
+  else if (Cin <= 8)
+    stem_bwd7_kernel<8, 8><<<grid, SB_THREADS, 0, stream>>>(v, w, Cin, dx);
+  else
+    stem_bwd7_kernel<16, 4><<<grid, SB_THREADS, 0, stream>>>(v, w, Cin, dx);
+  FFCB_LAUNCH_CHECK("stem_bwd7_kernel");
+  return FFCB_OK;
+}
 
 int relu_bwd(const ffcb_tensor* dy, const ffcb_tensor* y, const ffcb_tensor* out, cudaStream_t stream) {
   int rc;

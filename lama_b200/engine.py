@@ -1168,6 +1168,9 @@ def build_module_program(module, kind: str, shapes: Sequence[Optional[Tuple[int,
         build_generator_program(prog, module, shapes[0])
     elif kind == "generator_rear_grad":
         build_rear_grad_program(prog, module, shapes[0], shapes[1])
+    elif kind == "generator_grad":                        # the whole generator, forward + input gradient
+        from .generator_grad import build_generator_grad_program
+        build_generator_grad_program(prog, module, shapes[0])
     elif kind == "generator_rear":                       # the rear's forward alone (lowest refinement scale)
         emit_rear_forward(prog, module, shapes[0], shapes[1])
     elif kind.startswith("generator_refine:"):          # "generator_refine:<H0>x<W0>" (crop of the prediction)
@@ -1385,11 +1388,18 @@ def emit_rear_forward(prog: Program, gen, sl: Tuple[int, ...], sg: Tuple[int, ..
     back), X <- X + Y2 (ffcb_add); then the generator program's tail.  Returns what the backward reads."""
     _stem, _downs, _blocks, ups, _out_blk, head, out_act = _generator_layout(gen)
     X, saved = emit_rear_blocks(prog, gen, sl, sg)
+    ups_out = emit_rear_tail(prog, ups, head, out_act, X)
+    return dict(sl=tuple(sl), sg=tuple(sg), saved=saved, ups_out=ups_out)
+
+
+def emit_rear_tail(prog: Program, ups, head, out_act: int, X: Buf) -> List[Buf]:
+    """The up-sampling tail and head of the forward+backward programs from the bottleneck buffer ``X`` to the output
+    y0; returns every up stage's ReLU output (``emit_up_tail``)."""
     H, W = X.H * 2 ** len(ups), X.W * 2 ** len(ups)
     ups_out = emit_up_tail(prog, ups, X, _tc_head(prog, head, H, W))
     emit_head(prog, head, out_act, ups_out[-1], _tc_head(prog, head, H, W))
-    prog.outputs["y0"] = (sl[0], head.out_channels, H, W)
-    return dict(sl=tuple(sl), sg=tuple(sg), saved=saved, ups_out=ups_out)
+    prog.outputs["y0"] = (X.B, head.out_channels, H, W)
+    return ups_out
 
 
 def emit_rear_blocks(prog: Program, gen, sl: Tuple[int, ...], sg: Tuple[int, ...]) -> Tuple[Buf, list]:
@@ -1402,13 +1412,21 @@ def emit_rear_blocks(prog: Program, gen, sl: Tuple[int, ...], sg: Tuple[int, ...
     X = prog.buf("in", b, h, w, cl + cg, gemm=True, halo=True)
     prog.ops.append(ToNHWC("x0", TV(X, 0, cl)))
     prog.ops.append(ToNHWC("x1", TV(X, cl, cg)))
+    return X, emit_block_chain(prog, blocks, X, X, cl, cg)
+
+
+def emit_block_chain(prog: Program, blocks, X: Buf, out: Buf, cl: int, cg: int) -> list:
+    """The residual blocks of a forward+backward program on ``X``: per block conv1 -> Y1, conv2 -> its own Y2, then
+    the identity add (ffcb_add) into ``out`` — ``X`` itself runs them in place; another buffer keeps ``X`` (a ReLU
+    output the backward reads) and takes the later blocks in place.  Returns (block, Y1, Y2) per block."""
     saved = []
     for blk in blocks:
         Y1, _, _ = emit_ffc_bn_act(prog, blk.conv1, X, cl, cg)
         Y2, _, _ = emit_ffc_bn_act(prog, blk.conv2, Y1, cl, cg)
-        prog.ops.append(AddOp(TV(X), TV(Y2), TV(X)))
+        prog.ops.append(AddOp(TV(X), TV(Y2), TV(out)))
         saved.append((blk, Y1, Y2))
-    return X, saved
+        X = out
+    return saved
 
 
 def emit_rear_backward(prog: Program, gen, fwd: dict, dy: str):
@@ -1418,8 +1436,14 @@ def emit_rear_backward(prog: Program, gen, fwd: dict, dy: str):
     own weight [Cin, Cout, 3, 3] (no flip) and the BN scale folded along its input axis, then the ReLU mask of the stage
     below -> the blocks in reverse, each as two FFC_BN_ACT backwards with the identity path added by the second."""
     _stem, _downs, _blocks, ups, _out_blk, head, out_act = _generator_layout(gen)
-    sl, sg, saved, ups_out = fwd["sl"], fwd["sg"], fwd["saved"], fwd["ups_out"]
-    b = sl[0]
+    DX = emit_tail_backward(prog, ups, head, out_act, fwd["ups_out"], dy)
+    emit_rear_blocks_backward(prog, fwd["saved"], DX, fwd["sl"], fwd["sg"])
+
+
+def emit_tail_backward(prog: Program, ups, head, out_act: int, ups_out: List[Buf], dy: str, gemm: bool = False) -> Buf:
+    """The head adjoint and the up stages' adjoints of ``emit_rear_backward``, from ``dy`` to the gradient w.r.t. the
+    bottleneck, returned as a new buffer (a contraction operand with ``gemm``)."""
+    b = ups_out[-1].B
     H, W = ups_out[-1].H, ups_out[-1].W
     dev = head.weight.device
     n = head.out_channels
@@ -1436,9 +1460,9 @@ def emit_rear_backward(prog: Program, gen, fwd: dict, dy: str):
             D = prog.buf("grad.dup", b, hi, wi, ct.in_channels, gemm=True)
             prog.ops.append(ReluBwdOp(TV(E_), TV(ups_out[k - 1]), TV(D)))
         else:
-            DX = prog.buf("grad.dx", b, hi, wi, ct.in_channels)
+            DX = prog.buf("grad.dx", b, hi, wi, ct.in_channels, gemm=gemm)
             prog.ops.append(ConvOp(pk, [TV(D), None], TV(DX), tag=f"grad: convT{k}^T (stride 2)"))
-    emit_rear_blocks_backward(prog, saved, DX, sl, sg)
+    return DX
 
 
 def pack_up_adjoint(ct, bn, dev) -> P.PackedConv:
@@ -1452,11 +1476,18 @@ def pack_up_adjoint(ct, bn, dev) -> P.PackedConv:
 def emit_rear_blocks_backward(prog: Program, saved: list, DX: Buf, sl: Tuple[int, ...], sg: Tuple[int, ...]):
     """The residual blocks' part of the rear backward, from the bottleneck gradient ``DX`` to the outputs dx0, dx1."""
     cl, cg = sl[1], sg[1]
+    DX = emit_block_chain_backward(prog, saved, DX, cl, cg)
+    prog.ops.append(ToNCHW(TV(DX, 0, cl), "dx0")); prog.outputs["dx0"] = tuple(sl)
+    prog.ops.append(ToNCHW(TV(DX, cl, cg), "dx1")); prog.outputs["dx1"] = tuple(sg)
+
+
+def emit_block_chain_backward(prog: Program, saved: list, DX: Buf, cl: int, cg: int) -> Buf:
+    """The backward of ``emit_block_chain`` from the gradient ``DX`` w.r.t. its output: each block as two FFC_BN_ACT
+    backwards, the identity path added by the second.  Returns the gradient w.r.t. the chain's input."""
     for blk, Y1, Y2 in reversed(saved):
         D1 = emit_ffc_bn_act_backward(prog, blk.conv2, Y2, TV(DX), cl, cg)
         DX = emit_ffc_bn_act_backward(prog, blk.conv1, Y1, TV(D1), cl, cg, extra=TV(DX))
-    prog.ops.append(ToNCHW(TV(DX, 0, cl), "dx0")); prog.outputs["dx0"] = tuple(sl)
-    prog.ops.append(ToNCHW(TV(DX, cl, cg), "dx1")); prog.outputs["dx1"] = tuple(sg)
+    return DX
 
 
 def refine_supported(gen, shape_l, shape_g, crop: Tuple[int, int]) -> bool:
@@ -1917,18 +1948,19 @@ def get_executor(module, kind: str, tensors, math: Optional[int] = None,
 class _SplitProgramFn(torch.autograd.Function):
     """Native forward AND native input gradients through a forward+backward program, weights frozen — what the
     reference's refinement loop (evaluation/refinement.py:137-167) needs: ``resnet_block_grad`` for one FFCResnetBlock
-    (SURVEY.md row f3), ``generator_rear_grad`` for the whole rear (residual blocks, up-sampling tail, head).
-    Forward runs part 0 on inputs x0, x1 and returns the program outputs ``ys`` (plus x0 / x1 with ``residual``: the block
+    (SURVEY.md row f3), ``generator_rear_grad`` for the whole rear (residual blocks, up-sampling tail, head);
+    ``generator_grad`` for the whole generator (input x0 alone).
+    Forward runs part 0 on inputs x0[, x1] and returns the program outputs ``ys`` (plus x0 / x1 with ``residual``: the block
     program leaves the identity add to the caller); backward runs part 1 on one gradient g<i> per output.  The forward's
     activations stay in the executor's buffers, one executor per (module, shape): a second forward before the backward
     of the first would overwrite them, which raises instead of returning wrong gradients."""
 
     @staticmethod
-    def forward(ctx, module, kind, ys, residual, what, x0, x1):
-        ex = get_executor(module, kind, (x0, x1))
-        xs = (x0.detach().contiguous(), x1.detach().contiguous())
-        outs = ex.run({"x0": xs[0], "x1": xs[1]}, part=0)
-        ctx.ex, ctx.generation, ctx.what = ex, ex.generation, what
+    def forward(ctx, module, kind, ys, residual, what, *xs):
+        ex = get_executor(module, kind, xs)
+        xs = tuple(x.detach().contiguous() for x in xs)
+        outs = ex.run({f"x{i}": x for i, x in enumerate(xs)}, part=0)
+        ctx.ex, ctx.generation, ctx.what, ctx.n_in = ex, ex.generation, what, len(xs)
         res = tuple(x + outs[y] if residual else outs[y].clone() for y, x in zip(ys, xs))
         return res if len(res) > 1 else res[0]
 
@@ -1939,7 +1971,7 @@ class _SplitProgramFn(torch.autograd.Function):
             raise RuntimeError(f"lama_b200: {ctx.what} ran forward again (same shape) before this backward; "
                                "its saved activations were overwritten")
         outs = ex.run({f"g{i}": g.contiguous() for i, g in enumerate(grads)}, part=1)
-        return None, None, None, None, None, outs["dx0"].clone(), outs["dx1"].clone()
+        return (None,) * 5 + tuple(outs[f"dx{i}"].clone() for i in range(ctx.n_in))
 
 
 def block_with_input_grad(module, x_l, x_g):
@@ -1951,6 +1983,19 @@ def generator_rear_with_input_grad(gen, z1, z2):
     """pred = ``gen.model[first_block:]((z1, z2))`` on the native path, differentiable w.r.t. z1 / z2 (the weights are
     frozen).  Callers check ``rear_grad_supported(gen, z1.shape, z2.shape)`` first."""
     return _SplitProgramFn.apply(gen, "generator_rear_grad", ("y0",), False, "the generator's rear", z1, z2)
+
+
+def generator_grad_supported(gen, shape) -> bool:
+    """The whole generator has a native forward + input-gradient program (kind ``generator_grad``) for inputs of
+    ``shape``: ``lama_b200.generator_grad.generator_grad_supported``."""
+    from .generator_grad import generator_grad_supported as supported
+    return supported(gen, shape)
+
+
+def generator_with_input_grad(gen, x):
+    """``gen(x)`` on the native path, differentiable w.r.t. x (the weights are frozen).  Callers check
+    ``generator_grad_supported(gen, x.shape)`` first."""
+    return _SplitProgramFn.apply(gen, "generator_grad", ("y0",), False, "the generator", x)
 
 
 def run_module(module, kind: str, tensors):

@@ -54,6 +54,22 @@ def _native_ok(*tensors) -> bool:
     return any(torch.is_tensor(t) for t in tensors)
 
 
+def _generator_grad_native(gen, x) -> bool:
+    """Autograd is on, the generator is in eval mode with frozen weights and gets a CUDA float32 input: the native
+    path of the whole generator under autograd applies (``LAMA_B200_NATIVE_GRAD=0`` disables it)."""
+    return (torch.is_grad_enabled() and not gen.training and not torch.jit.is_tracing() and torch.is_tensor(x)
+            and x.is_cuda and x.dtype == torch.float32 and os.environ.get("LAMA_B200_NATIVE_GRAD", "1") != "0"
+            and _engine.generator_grad_supported(gen, tuple(x.shape)))
+
+
+def _generator_grad_forward(gen, x):
+    """``gen(x)`` under autograd on the native path: the forward + input-gradient program when x wants a gradient
+    (a second forward of the same shape before its backward raises), else the no-grad generator program."""
+    if x.requires_grad:
+        return _engine.generator_with_input_grad(gen, x)
+    return _engine.run_module(gen, "generator", (x,))[0]
+
+
 def _fallback(why: str):
     if os.environ.get("LAMA_B200_STRICT") == "1" and not torch.jit.is_tracing():
         raise RuntimeError(f"lama_b200: native path unavailable ({why}) and LAMA_B200_STRICT=1")
@@ -410,6 +426,8 @@ class FFCResNetGenerator(nn.Module):
     def forward(self, input):
         if _native_ok(input) and not self.training and _engine.generator_supported(self, input):
             return _engine.run_module(self, "generator", (input,))[0]
+        if _generator_grad_native(self, input):
+            return _generator_grad_forward(self, input)
         if (torch.jit.is_tracing() and self._ffcb_spec is not None and not self.training and torch.is_tensor(input)
                 and input.is_cuda and input.dtype == torch.float32 and not torch.is_grad_enabled()
                 and os.environ.get("LAMA_B200_TRACE_NATIVE", "1") == "1" and _engine.generator_supported(self, input)):

@@ -155,6 +155,43 @@ def pack_conv_transpose_phases(weight: torch.Tensor, bias: Optional[torch.Tensor
     return out
 
 
+def pack_down_adjoint_phases(weight: torch.Tensor, scale: torch.Tensor, *, padded: bool,
+                             device=None) -> List[Tuple[int, int, PackedConv]]:
+    """The adjoint of a 3x3, stride-2, pad-1 convolution with the BN ``scale`` folded (``y = scale * conv(x)``) w.r.t.
+    its input, as four sub-pixel phase contractions of the output gradient g (H/2 x W/2, zero outside).  weight:
+    [N, C, 3, 3]; every phase is a stride-1, zero-border contraction N -> C.  Input position u of the padded axis
+    receives g[i] w[ky] for u = 2i + ky:
+      ``padded``: the (H+2)-long padded axis, phase (2p+a) of size H/2 + 1 (ring included), to be folded by the
+                  reflection's adjoint:   a == 0: (ky=0, di=0), (ky=2, di=-1)     a == 1: (ky=1, di=0)
+      else:       the interior only (zero padding: the ring's gradient is dropped), phase size H/2 — the phases of
+                  ConvTranspose2d(k3, s2, p1, op1):  a == 0: (ky=1, di=0)       a == 1: (ky=2, di=0), (ky=0, di=+1)
+    Returns [(a, b, PackedConv)]."""
+    w = weight.detach().double() * scale.double()[:, None, None, None]      # [N, C, 3, 3]
+    n, c = w.shape[0], w.shape[1]
+    sel = {0: [(0, 0), (2, -1)], 1: [(1, 0)]} if padded else {0: [(1, 0)], 1: [(2, 0), (0, 1)]}
+    out = []
+    for a in (0, 1):
+        for b in (0, 1):
+            segs, cols = [], []
+            for ky, di in sel[a]:
+                for kx, dj in sel[b]:
+                    segs.append(Seg(0, di, dj, 0, n))
+                    cols.append(w[:, :, ky, kx].t())                   # [C, N]
+            w_kn = torch.cat(cols, dim=1).t().contiguous().float()
+            if device is not None:
+                w_kn = w_kn.to(device)
+            out.append((a, b, PackedConv(segs=segs, n_out=c, w_kn=w_kn, shift=None, stride=1, border=L.BORDER_ZERO,
+                                         act=L.ACT_NONE)))
+    return out
+
+
+def pack_stem_adjoint(weight: torch.Tensor, scale: torch.Tensor, device=None) -> torch.Tensor:
+    """7x7 stem weight [N, Cin, 7, 7] with the BN scale folded -> float [N][7*7][Cin] (ffcb_stem_bwd7)."""
+    w = weight.detach().double() * scale.double()[:, None, None, None]
+    w = w.permute(0, 2, 3, 1).reshape(w.shape[0], 49, w.shape[1]).contiguous().float()
+    return w.to(device) if device is not None else w
+
+
 def pack_stem(weight: torch.Tensor, scale: torch.Tensor, shift: torch.Tensor, device=None):
     """7x7 stem (ffc.py:316): [N, Cin, 7, 7] -> float [(ky*7+kx)*Cin + c][N], BN folded."""
     w = weight.detach().double() * scale.double()[:, None, None, None]

@@ -23,7 +23,8 @@ from functools import partial
 import torch.nn as nn
 
 from . import engine as _engine
-from .modules import FFCResnetBlock, _fallback, _native_ok, get_activation
+from .modules import (FFCResnetBlock, _fallback, _generator_grad_forward, _generator_grad_native, _native_ok,
+                      get_activation)
 
 __all__ = ["ResnetBlock", "GlobalGenerator", "reference_only_options"]
 
@@ -179,5 +180,7 @@ class GlobalGenerator(nn.Module):
     def forward(self, input):
         if _native_ok(input) and not self.training and _engine.generator_supported(self, input):
             return _engine.run_module(self, "generator", (input,))[0]
+        if _generator_grad_native(self, input):
+            return _generator_grad_forward(self, input)
         _fallback("GlobalGenerator options / mode")
         return self.model(input)
